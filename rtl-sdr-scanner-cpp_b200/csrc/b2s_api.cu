@@ -358,13 +358,8 @@ static int make_tile_map(CUtensorMap* out, const float* base, size_t cols, size_
   const cuuint64_t strides[1] = {cols * sizeof(float)};
   const cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
   const cuuint32_t elem[2] = {1, 1};
-  CUtensorMapL2promotion promo = CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
-  if (const char* e = getenv("B2S_K2_L2PROMO")) {  // A/B measurements
-    const int v = atoi(e);
-    promo = v == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : v == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : v == 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : promo;
-  }
   const CUresult r = encode(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, elem, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                            CU_TENSOR_MAP_SWIZZLE_NONE, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(B2S_E_CUDA, "cuTensorMapEncodeTiled failed (%d) for box %dx%d", static_cast<int>(r), box_cols, box_rows);
   return 0;
 }
@@ -1032,7 +1027,7 @@ int b2s_recorder_create(b2s_engine* e, int32_t sample_rate_hz, int32_t bandwidth
     if (st.hc > 4096) rc = fail(B2S_E_INVALID, "resampler stage %d/%d needs %d samples of history", st.interp, st.decim, st.hc);
     if (!rc) rc = st.taps.alloc(st.n_taps);
     if (!rc && cudaMemcpy(st.taps.p, st.h_taps.data(), sizeof(float) * st.n_taps, cudaMemcpyHostToDevice) != cudaSuccess) rc = fail(B2S_E_CUDA, "taps upload failed");
-    if (!rc && st.interp == 1 && st.decim >= 2 && (st.n_taps + st.decim - 1) / st.decim <= kPolyQ && !getenv("B2S_RECORDER_GENERIC")) {
+    if (!rc && st.interp == 1 && st.decim >= 2 && (st.n_taps + st.decim - 1) / st.decim <= kPolyQ) {
       std::vector<float> pq(static_cast<size_t>(st.decim) * kPolyQ, 0.0f);  // h[q D + p] at [p][q], zero padded
       for (int k = 0; k < st.n_taps; ++k) pq[static_cast<size_t>(k % st.decim) * kPolyQ + k / st.decim] = st.h_taps[k];
       rc = st.taps_pq.alloc(pq.size());

@@ -16,7 +16,6 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
@@ -65,16 +64,6 @@ __device__ __forceinline__ void tma_load_2d(void* dst_smem, const void* tensor_m
                : "memory");
 }
 
-// 16-byte asynchronous copy global -> shared through the LSU (SASS LDGSTS); src_bytes < 16 zero-fills the rest (0: no global read)
-__device__ __forceinline__ void cp_async_16(void* dst_smem, const void* src_gmem, int src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(src_bytes) : "memory");
-}
-// the executing thread's arrival on `bar` is triggered when all its prior cp.async operations have completed (the barrier's
-// expected count includes it: .noinc)
-__device__ __forceinline__ void cp_async_mbar_arrive(uint64_t* bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
 // ---------------------------------------------------------------------------------------------------------
 // complex helpers
 // ---------------------------------------------------------------------------------------------------------
@@ -84,13 +73,6 @@ __device__ __forceinline__ float2 cmul(float2 a, float2 w) { return make_float2(
 __device__ __forceinline__ float2 mul_mi(float2 a) { return make_float2(a.y, -a.x); }  // a * (-i)
 __device__ __forceinline__ float2 cneg(float2 a) { return make_float2(-a.x, -a.y); }
 __device__ __forceinline__ float2 cscale(float2 a, float s) { return make_float2(a.x * s, a.y * s); }
-__device__ __forceinline__ float2 cmake(float2, float re, float im) { return make_float2(re, im); }  // (tag, re, im): construct a value of the tag's type
-// acc + a * w with the reference-free but fixed operation order of the split pre-pass (spectral3.cuh)
-__device__ __forceinline__ float2 cmadd(float2 a, float2 w, float2 acc) {
-  return make_float2(fmaf(a.x, w.x, fmaf(-a.y, w.y, acc.x)), fmaf(a.x, w.y, fmaf(a.y, w.x, acc.y)));
-}
-__device__ __forceinline__ float cre(float2 a) { return a.x; }
-__device__ __forceinline__ float cim(float2 a) { return a.y; }
 
 // ---------------------------------------------------------------------------------------------------------
 // cpk: complex value whose arithmetic is fixed half by half — every half is one IEEE round-to-nearest add, sub, mul or fma

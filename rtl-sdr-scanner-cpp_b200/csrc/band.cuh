@@ -358,10 +358,6 @@ struct b2s_band : public DeviceQueries {
         }
         if (!detect_bins && 112 % d == 0 && 112 + 2 * hp <= kSumThreads) detect_bins = 112;
       }
-      if (const char* e = getenv("B2S_K2_BINS")) {  // A/B measurements
-        const int bins = atoi(e);
-        if (bins > 0 && bins <= kDetectBinsPerCta && bins % kBoxSegment == 0 && bins % d == 0 && bins + 2 * hp <= kSumThreads) detect_bins = bins;
-      }
       if (!detect_bins)
         return fail(B2S_E_INVALID, "grouping_x %d (halo %d bins per side) with a spectrogram decimation of %d does not fit a K2 CTA of %d columns", c.grouping_x, hp, d, kSumThreads);
     }
@@ -798,9 +794,6 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
   da.spec_rows = s.spec_rows.p;
   da.box_last = s.host_track ? nullptr : s.box_last.p;
   da.cta_ns = nullptr;
-  da.trace_cta = -1;
-  if (const char* e = getenv("B2S_K2_TRACE_CTA")) da.trace_cta = atoi(e);
-  if (const char* e = getenv("B2S_K2_TRACE_SEG")) da.trace_seg = atoi(e);
   if (profiling && profile_ctas) {
     if ((rc = s.cta_ns.alloc(2 * ((n + detect_bins - 1) / detect_bins)))) return rc;
     da.cta_ns = s.cta_ns.p;
@@ -817,7 +810,6 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
     const size_t fixed = sizeof(float) * (kAvgBuffers * width * (kDetectTileFrames + 1) + kBoxGroups * kDetectBinsPerCta * kDetectTileFrames);
     const size_t per_tile = sizeof(float) * kDetectTileFrames * width;
     da.n_buffers = static_cast<int>(std::min<size_t>(kDetectBuffers, (kSmemBudget - fixed) / per_tile));
-    if (const char* e = getenv("B2S_K2_BUFFERS")) da.n_buffers = std::max(2, std::min(da.n_buffers, atoi(e)));  // experiments
     const size_t smem = fixed + per_tile * da.n_buffers;
     const int grid = (n + detect_bins - 1) / detect_bins;
     if ((rc = prepare_kernel(engine, k_detect<21, 10, 152>, kDetectThreads, 220 * 1024, nullptr))) return rc;
@@ -826,11 +818,11 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
     if ((rc = prepare_kernel(engine, k_detect<21, 10>, kDetectThreads, 220 * 1024, nullptr))) return rc;
     if ((rc = prepare_kernel(engine, k_detect<0, -1>, kDetectThreads, 220 * 1024, nullptr))) return rc;
     if (profiling) CU(cudaEventRecord(s.ev[2], stream));
-    if (half == 10 && Y == 21 && width == 152 && !getenv("B2S_K2_RUNTIME_WIDTH")) {
+    if (half == 10 && Y == 21 && width == 152) {
       k_detect<21, 10, 152><<<grid, kDetectThreads, smem, stream>>>(da, s.psd_map);  // N >= 16384 on 132 SMs: 128 bins + 2 x 12 halo columns
-    } else if (half == 10 && Y == 21 && width == 136 && !getenv("B2S_K2_RUNTIME_WIDTH")) {
+    } else if (half == 10 && Y == 21 && width == 136) {
       k_detect<21, 10, 136><<<grid, kDetectThreads, smem, stream>>>(da, s.psd_map);  // N = 8192: 112 bins + 2 x 12 halo columns
-    } else if (half == 10 && Y == 21 && width == 56 && !getenv("B2S_K2_RUNTIME_WIDTH")) {
+    } else if (half == 10 && Y == 21 && width == 56) {
       k_detect<21, 10, 56><<<grid, kDetectThreads, smem, stream>>>(da, s.psd_map);   // N = 4096: 32 bins + 2 x 12
     } else if (half == 10 && Y == 21) {
       k_detect<21, 10><<<grid, kDetectThreads, smem, stream>>>(da, s.psd_map);
@@ -886,7 +878,6 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
     ta.ring_before = d_ring[ring_in].p;
     ta.state = d_state.p;
     ta.result = s.d_result.p;
-    if (const char* e = getenv("B2S_TRACK_DEBUG")) ta.debug = atoi(e) >= 2;
     if ((rc = prepare_kernel(engine, k_track, kTrackThreads, sizeof(TrackShared), nullptr))) return rc;
     if (profiling) {
       for (auto& e : s.tev) {
@@ -959,9 +950,6 @@ int b2s_band::finish_chunk(PushSlot& s) {
     prof.track_evals += r.n_evals;
     prof.track_events += r.n_events;
     prof.track_best_index += r.n_best;
-    if (getenv("B2S_TRACK_DEBUG"))
-      fprintf(stderr, "[k_track] T=%d cycles %lld: runs %lld eval %lld walk %lld out %lld; evals %d events %d best %d entries %d\n", T, r.cycles, r.phase[0], r.phase[1], r.phase[2],
-              r.phase[3], r.n_evals, r.n_events, r.n_best, r.n_entries);
     overflow = worst_count > slot_capacity;
     std::vector<b2s_transmission> list(r.n_tx);
     std::memcpy(list.data(), r.tx, sizeof(b2s_transmission) * std::min(r.n_tx, B2S_MAX_TX));
@@ -1032,13 +1020,6 @@ int b2s_band::finish_chunk(PushSlot& s) {
       CU(cudaStreamSynchronize(st));
       std::vector<double> dur(grid);
       for (int i = 0; i < grid; ++i) dur[i] = static_cast<double>(ns[2 * i + 1] - ns[2 * i]) * 1e-6;
-      if (getenv("B2S_K2_DUMP_CTAS")) {  // diagnostics: start (relative to the first CTA) and run time of every CTA, in microseconds
-        unsigned long long first = ~0ull;
-        for (int i = 0; i < grid; ++i) first = std::min(first, ns[2 * i]);
-        fprintf(stderr, "[k_detect ctas]");
-        for (int i = 0; i < grid; ++i) fprintf(stderr, " %d:%.1f+%.1f", i, static_cast<double>(ns[2 * i] - first) * 1e-3, dur[i] * 1e3);
-        fprintf(stderr, "\n");
-      }
       std::sort(dur.begin(), dur.end());
       prof.detect_cta_median_ms += dur[grid / 2];
       prof.detect_cta_max_ms += dur[grid - 1];

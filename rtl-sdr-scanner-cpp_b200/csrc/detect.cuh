@@ -14,7 +14,6 @@
 // 16 bins changes rounding only (<= 1e-3 dB vs the reference's own drift, asserted in tests) and keeps the work
 // parallel. b2s_average(..., exact=1) provides the serial form for operator-level bit parity.
 #pragma once
-#include <cstdio>
 #include <cstring>
 
 #include "b2s_device.cuh"
@@ -95,7 +94,6 @@ struct DetectArgs {
   int emit_div[kMaxSpecEmits];     // Container::m_counter at that moment
   signed char* spec_rows;          // [n_emit][M]
   unsigned long long* cta_ns;      // optional [2 * grid]: %globaltimer at CTA start / end (profiling: load balance)
-  int trace_cta, trace_seg;        // trace_cta >= 0: this CTA prints where its SUM warp 0 and box warp (group 0, segment trace_seg) spend their cycles
   float* box_last;  // optional [N]: the boxcar row of the push's last frame (K4 reads the signals' m_power from it)
   // optional dense rows [T][N]
   float* dense_q;
@@ -211,10 +209,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) { asm volatile("mbarr
 // Warp roles of k_detect. One CTA owns kDetectBinsPerCta bins plus a halo of X/2 bins (rounded up to 4) on each side,
 // computed redundantly; every role walks the push in tiles of kDetectTileFrames frames and the roles meet only through
 // mbarriers, so each runs as far ahead as its buffers allow.
-#ifndef B2S_K2_BOX_GROUPS
-#define B2S_K2_BOX_GROUPS 2
-#endif
-constexpr int kBoxGroups = B2S_K2_BOX_GROUPS;  // box-warp groups; group g takes the tiles with (tile % kBoxGroups) == g (1 or 2)
+constexpr int kBoxGroups = 2;  // box-warp groups; group g takes the tiles with (tile % kBoxGroups) == g
 constexpr int kSumWarps = 5, kBoxWarps = kDetectBinsPerCta / kBoxSegment;
 constexpr int kSumThreads = 32 * kSumWarps;    // one thread per column (<= 160 columns: the CTA's bins plus both halos)
 constexpr int kBoxThreads = 32 * kBoxWarps;    // threads of ONE box group: one warp per boxcar segment, lane = frame of the tile
@@ -223,69 +218,24 @@ constexpr int kSpecThreads = 32 * kSpecWarps;
 constexpr int kDetectThreads = kSumThreads + 32 /*producer*/ + kBoxGroups * kBoxThreads + kSpecThreads;
 // Role of every warp. A CTA's warps are dealt round robin to the four SM sub-partitions (warp id % 4), each with its own issue
 // port. The SUM warps carry the kernel's only serial chain and never wait (profile: the box warps spend half their samples at the
-// FULL barrier), so their issue rate is the tile rate. The default uses contiguous role ranges — box, producer, SPEC, SUM — which
-// spreads the five SUM warps over all four sub-partitions; B2S_K2_ROLE_MAP=1 packs them three + two onto sub-partitions 0 and 1
-// beside the mostly sleeping warps (box warps on 2 and 3), for comparison.
-#ifndef B2S_K2_ROLE_MAP
-#define B2S_K2_ROLE_MAP 0
-#endif
+// FULL barrier), so their issue rate is the tile rate. The roles take contiguous warp ranges — box, producer, SPEC, SUM — which
+// spreads the five SUM warps over all four sub-partitions.
 enum : int { kRoleSum = 0, kRoleProducer = 1, kRoleSpec = 2, kRoleBox = 3 };
 struct WarpRole {
   int role, index;  // index: SUM warp 0..4 (columns 32 * index ...), SPEC warp 0..1, box: group * kBoxWarps + segment
 };
-static_assert(kSumWarps == 5 && kSpecWarps == 2 && kBoxGroups == 2 && kBoxWarps == 8, "the role table below is written for 24 warps");
 __device__ __forceinline__ WarpRole warp_role(int wid) {
-#if B2S_K2_ROLE_MAP
-  // sub-partition 0: wid 0 4 8 12 16 20   1: wid 1 5 9 13 17 21   2: wid 2 6 10 14 18 22   3: wid 3 7 11 15 19 23
-  switch (wid) {
-    case 0: return {kRoleSum, 0};
-    case 4: return {kRoleSum, 1};
-    case 8: return {kRoleSum, 2};
-    case 1: return {kRoleSum, 3};
-    case 5: return {kRoleSum, 4};
-    case 9: return {kRoleProducer, 0};
-    case 13: return {kRoleSpec, 0};
-    case 17: return {kRoleSpec, 1};
-    case 12: return {kRoleBox, 0 * kBoxWarps + 7};  // segment 7 of each group: idle when a CTA owns 112 bins
-    case 16: return {kRoleBox, 1 * kBoxWarps + 7};
-    case 20: return {kRoleBox, 0 * kBoxWarps + 6};
-    case 21: return {kRoleBox, 1 * kBoxWarps + 6};
-    default: {  // sub-partitions 2 and 3: wid = 4 q + 2 + h, q = 0..5, h = 0..1 -> twelve box warps: segments 0..5 of both groups
-      const int q = wid >> 2, h = (wid & 3) - 2;  // h: 0 / 1
-      const int k = 2 * q + h;                    // 0..11
-      return {kRoleBox, (k & 1) * kBoxWarps + (k >> 1)};
-    }
-  }
-#else
   if (wid < kBoxGroups * kBoxWarps) return {kRoleBox, wid};
   if (wid == kBoxGroups * kBoxWarps) return {kRoleProducer, 0};
   if (wid < kBoxGroups * kBoxWarps + 1 + kSpecWarps) return {kRoleSpec, wid - kBoxGroups * kBoxWarps - 1};
   return {kRoleSum, wid - kBoxGroups * kBoxWarps - 1 - kSpecWarps};
-#endif
 }
 // registers per thread: 24 warps, 6 per sub-partition (16384 registers each): 6 x 32 x 80 = 15360
 constexpr int kDetectRegs = 80;
 // the register file is split over the 4 SM sub-partitions (16384 registers each) and a CTA's warps are dealt round robin
 static_assert(((kDetectThreads / 32 + 3) / 4) * ((kDetectRegs * 32 + 511) / 512 * 512) <= 16384, "k_detect must fit the register file");
 static_assert(kDetectBinsPerCta / 2 <= kSpecThreads, "one SPEC thread per spectrogram column of a CTA");
-#ifndef B2S_K2_CPASYNC
-#define B2S_K2_CPASYNC 0  // PSD tiles through one 2-D TMA load per tile (0) or 16-byte cp.async chunks (1: for comparison)
-#endif
-#ifndef B2S_K2_DIAG
-#define B2S_K2_DIAG 0  // timing diagnostics only (wrong results): 1 = box warps skip the division and the boxcar, 2 = SUM warps skip the march
-#endif
-#ifndef B2S_K2_TRACE
-#define B2S_K2_TRACE 0  // 1: the per-role cycle trace (DetectArgs::trace_cta) is compiled in. It costs the traced roles ~16 registers of 64-bit
-                        // counters under the 80-register cap, so the shipped kernel leaves it out; build with -DB2S_K2_TRACE=1 to use it
-#endif
-constexpr bool kTrace = B2S_K2_TRACE != 0;
-#ifndef B2S_K2_EARLY_EMPTY
-#define B2S_K2_EARLY_EMPTY 1
-#endif
-#ifndef B2S_K2_AVG_BUFFERS
-#define B2S_K2_AVG_BUFFERS 2
-#endif
-constexpr int kAvgBuffers = B2S_K2_AVG_BUFFERS;  // average tiles between the SUM and the box warps (a multiple of kBoxGroups)
+constexpr int kAvgBuffers = 2;  // average tiles between the SUM and the box warps (a multiple of kBoxGroups)
 static_assert(kAvgBuffers % kBoxGroups == 0 && kAvgBuffers <= 4, "each box group owns whole buffers; barrier ids 2..9");
 constexpr int kBarFull = 2, kBarEmpty = 2 + kAvgBuffers;  // hardware barriers (one pair per average buffer): waiting warps sleep instead of polling
 
@@ -337,9 +287,6 @@ __device__ __forceinline__ float spec_tile(const float* __restrict__ raw, int wi
 // 132 SMs; 136 = 112 bins + 2 x 12),
 // or 0 for the runtime value: with a constant the SUM warps' 32 tile loads per column take immediate offsets instead of 32 address
 // instructions on the kernel's critical warps.
-#ifndef B2S_K2_SPEC_INTERLEAVE
-#define B2S_K2_SPEC_INTERLEAVE 1  // the inline spectrogram chain is accumulated branch-free, so ptxas can fill the Averager chain's latency gaps with it
-#endif
 template <int Y_T, int HALF_T, int WIDTH_T = 0>
 __global__ void __maxnreg__(kDetectRegs) k_detect(const DetectArgs a, const __grid_constant__ CUtensorMap psd_map) {
   extern __shared__ __align__(128) float sm[];
@@ -384,7 +331,7 @@ __global__ void __maxnreg__(kDetectRegs) k_detect(const DetectArgs a, const __gr
     }
     rel_n = cnt;
     for (int i = 0; i < a.n_buffers; ++i) {
-      mbar_init(&p_full[i], B2S_K2_CPASYNC ? 32 : 1);  // cp.async: one arrival per producer lane when its copies have landed; TMA: one + the bytes
+      mbar_init(&p_full[i], 1);  // the producer's arrival + the bytes of its TMA load
       mbar_init(&p_empty[i], kSumWarps + ((a.spec_out > 0 && n / a.spec_out > 1) ? kSpecWarps : 0));  // the SPEC warps only run for decimating spectrograms
     }
     fence_barrier_init();
@@ -426,9 +373,6 @@ __global__ void __maxnreg__(kDetectRegs) k_detect(const DetectArgs a, const __gr
 
     int ps = 0;            // PSD ring slot of the current tile and the parity of its mbarrier phase
     uint32_t ps_phase = 0;
-    const bool tr = kTrace && a.trace_cta == static_cast<int>(blockIdx.x) && ct == 0;
-    long long tr_c[4] = {0, 0, 0, 0};
-    const long long tr_begin = tr ? clock64() : 0;
     for (int tile = 0; tile < n_tiles; ++tile) {
       const int t0 = tile * TF;
       const int tf = min(TF, T - t0);
@@ -436,44 +380,29 @@ __global__ void __maxnreg__(kDetectRegs) k_detect(const DetectArgs a, const __gr
       const float* __restrict__ cur = psd_tiles + ps * tile_elems + ct;
       float* __restrict__ sum_col = sum_tiles + sb * sum_elems + ct * kSumPitch;  // my column of the transposed tile
       const bool steady = tile >= first_steady && tf == TF;  // the previous tile was full, so `lead` is valid
-      const long long c0 = tr ? clock64() : 0;
       mbar_wait_sleepy(&p_full[ps], ps_phase);                              // the PSD tile has landed
-      const long long c1 = tr ? clock64() : 0;
       if (tile >= kAvgBuffers) bar_sync(kBarEmpty + sb, kSumThreads + kBoxThreads);  // the box warps are done with this average buffer
-      const long long c2 = tr ? clock64() : 0;
       float q[TF];
       float checkpoint = 0.0f;
       // a spectrogram row completes inside this tile: one bit per tile, set by the host (a scan of the emission table with its
       // indexed constant loads sat on the serial chain's warps every tile)
       const bool emits = tile == emit_tile;
       const bool spec_inline = steady && d == 1 && !emits;
-#if B2S_K2_DIAG == 2
       if (steady) {
-      } else if (false) {
-#else
-      if (steady) {
-#endif
         if (active) {
           checkpoint = sum;  // m_sum before frame t0
           // two halves: the second half of the tile is loaded only when most of `lead` is dead, which keeps the live set at
           // ~40 frame values instead of 53 (no spills on the serial chain)
           constexpr int kSplit = TF / 2, kLate = kSplit - 4;
           const bool spec_here = spec_inline && spec_owner;
-#if B2S_K2_SPEC_INTERLEAVE
-          float sp = spec;  // accumulated by every thread, kept by the owners of an inline tile: no branch around the second chain
-#endif
+          // the spectrogram chain is accumulated by every thread and kept by the owners of an inline tile: with no branch around
+          // it, ptxas can fill the Averager chain's latency gaps with it
+          float sp = spec;
           auto load_half = [&](int f0) {
 #pragma unroll
             for (int f = f0; f < f0 + kSplit; ++f) q[f] = cur[f * width];
-#if B2S_K2_SPEC_INTERLEAVE
 #pragma unroll
             for (int f = f0; f < f0 + kSplit; ++f) sp = __fadd_rn(sp, q[f]);
-#else
-            if (spec_here) {
-#pragma unroll
-              for (int f = f0; f < f0 + kSplit; ++f) spec = __fadd_rn(spec, q[f]);
-            }
-#endif
 #pragma unroll
             for (int f = f0; f < f0 + kSplit; ++f) q[f] = __fsub_rn(q[f], thr);  // NoiseLearner::work, noise_learner.cpp:54
           };
@@ -491,9 +420,7 @@ __global__ void __maxnreg__(kDetectRegs) k_detect(const DetectArgs a, const __gr
           asm volatile("" ::: "memory");  // keep the compiler from hoisting the second half's loads to the top
           load_half(kSplit);
           march(kLate, TF);
-#if B2S_K2_SPEC_INTERLEAVE
           spec = spec_here ? sp : spec;
-#endif
         }
       } else if (active) {
         // ---- generic march (learning frames, first tile of a push, partial tiles, dense debug rows, runtime Y) ----
@@ -535,14 +462,7 @@ __global__ void __maxnreg__(kDetectRegs) k_detect(const DetectArgs a, const __gr
       if (ct == 0) tile_raw[sb] = steady ? 1 : 0;
       // (no fence: the barrier instruction orders this warp's shared-memory stores before the waiting warps' loads — the
       // producer / consumer pattern of the PTX manual; MEMBAR.SC.CTA here also waited for the warp's global stores)
-      const long long c3 = tr ? clock64() : 0;
       bar_arrive(kBarFull + sb, kSumThreads + kBoxThreads);  // hand the tile of averages to the box warps
-      if (tr) {
-        tr_c[0] += c1 - c0;
-        tr_c[1] += c2 - c1;
-        tr_c[2] += c3 - c2;
-        tr_c[3] += clock64() - c3;
-      }
       if (spec_owner && !spec_inline) {  // tiles with an emission, non-steady tiles
         const float* __restrict__ raw = cur;
         for (int f = 0; f < tf; ++f) {
@@ -573,7 +493,6 @@ __global__ void __maxnreg__(kDetectRegs) k_detect(const DetectArgs a, const __gr
         for (int f = 0; f < YC; ++f) lead[f] = q[TF - YC + f];
       }
     }
-    if (tr) printf("[k_detect cta %d] SUM warp 0: total %lld cycles: wait tile %lld, wait EMPTY %lld, march %lld, arrive FULL %lld, rest %lld (%d tiles)\n", blockIdx.x, clock64() - tr_begin, tr_c[0], tr_c[1], tr_c[2], tr_c[3], clock64() - tr_begin - tr_c[0] - tr_c[1] - tr_c[2] - tr_c[3], n_tiles);
     if (spec_owner) a.spec_sum[j] = spec;
     if (owner) {
       a.threshold_out[j] = thr;
@@ -600,32 +519,15 @@ __global__ void __maxnreg__(kDetectRegs) k_detect(const DetectArgs a, const __gr
     // Streams the tile [32 frames][width columns] of the PSD rows at (col0, t0) into the ring. Columns left of bin 0 / right of bin
     // N-1 and rows past the push arrive as zeros (nobody reads them).
     // One 2-D TMA load per tile: the rows are only (bins + halo) floats long in a row-major [T][N] matrix, so the copy engine's
-    // per-request cost dominates whichever way a tile is fetched; one request per tile keeps that cost lowest. 16-byte cp.async
-    // chunks through the LSU (B2S_K2_CPASYNC=1) are kept for comparison.
+    // per-request cost dominates whichever way a tile is fetched; one request per tile keeps that cost lowest.
     int ps = 0;
     uint32_t ps_phase = 1;  // waiting for the "previous" phase passes at once during the first round
-#if B2S_K2_CPASYNC
-    const int chunks_per_row = width / 4, chunks = TF * chunks_per_row;
-#endif
     for (int tile = 0; tile < n_tiles; ++tile) {
       mbar_wait_sleepy(&p_empty[ps], ps_phase);  // the SUM (and SPEC) warps released the slot
-#if B2S_K2_CPASYNC
-      float* dst = psd_tiles + ps * tile_elems;
-      const int t0 = tile * TF;
-      for (int i = lane; i < chunks; i += 32) {
-        const int row = i / chunks_per_row, c4 = (i - row * chunks_per_row) * 4;
-        const int col = col0 + c4;
-        const bool inside = t0 + row < T && col >= 0 && col < n;  // hp and N are multiples of 4: a chunk is inside or outside as a whole
-        const float* src = psd + (inside ? static_cast<size_t>(t0 + row) * n + col : 0);
-        cp_async_16(dst + row * width + c4, src, inside ? 16 : 0);  // src-size 0: the 16 bytes are zero-filled
-      }
-      cp_async_mbar_arrive(&p_full[ps]);  // this lane's arrival fires when all its copies above have landed
-#else
       if (lane == 0) {
         mbar_arrive_expect_tx(&p_full[ps], static_cast<uint32_t>(tile_elems * sizeof(float)));
         tma_load_2d(psd_tiles + ps * tile_elems, &psd_map, col0, tile * TF, &p_full[ps]);
       }
-#endif
       if (++ps == a.n_buffers) {
         ps = 0;
         ps_phase ^= 1;
@@ -696,16 +598,11 @@ __global__ void __maxnreg__(kDetectRegs) k_detect(const DetectArgs a, const __gr
     static_assert(kBoxThreads / 32 == kDetectBinsPerCta / kBoxSegment && kDetectTileFrames == 32, "one box warp per segment, one lane per frame");
     const int b0 = seg * SEG, bin0 = j0 + b0;
     float* my_box = box_park + (group * kBoxWarps + seg) * SEG * TF + lane;  // [k * TF]: written and read by this lane only
-    static_assert(kBoxGroups == 1 || kBoxGroups == 2, "group g takes the tiles with tile % kBoxGroups == g");
-    const bool btr = kTrace && a.trace_cta == static_cast<int>(blockIdx.x) && group == 0 && btid == 32 * a.trace_seg;
-    long long btr_c[3] = {0, 0, 0};
     for (int tile = group; tile < n_tiles; tile += kBoxGroups) {
       const int t0 = tile * TF;
       const int tf = min(TF, T - t0);
       const int sb = tile % kAvgBuffers;
-      const long long b0c = btr ? clock64() : 0;
       bar_sync(kBarFull + sb, kSumThreads + kBoxThreads);  // the SUM warps have written this tile
-      const long long b1c = btr ? clock64() : 0;
       const float* avg_tile = sum_tiles + sb * sum_elems;
       const bool raw = tile_raw[sb] != 0;  // the SUM warps handed over m_sum: m_average = m_sum / Y is computed here
       const int f = lane, t = t0 + f;
@@ -723,26 +620,15 @@ __global__ void __maxnreg__(kDetectRegs) k_detect(const DetectArgs a, const __gr
           float w[SEG + 2 * H];
 #pragma unroll
           for (int i = 0; i < SEG + 2 * H; ++i) w[i] = avg_tile[(hp + b0 - H + i) * kSumPitch + f];  // columns outside [0, N) hold 0.0f
-#if B2S_K2_DIAG == 1
-          if (false) {
-#else
           if (raw) {
-#endif
 #pragma unroll
             for (int i = 0; i < SEG + 2 * H; ++i) w[i] = div_const_fast<YD>(w[i]);  // averager.cpp:52-60 (0 / Y = 0 for the zero extension)
-#if B2S_K2_EARLY_EMPTY
             // every value of the tile this lane needs has been read AND used: hand the buffer back before the serial boxcar chain, so
             // the SUM warps are not held up by it (with two average buffers they would otherwise wait for this warp's whole tile)
             if (tile + kAvgBuffers < n_tiles) bar_arrive(kBarEmpty + sb, kSumThreads + kBoxThreads);
             released = true;
-#endif
           }
-#if B2S_K2_DIAG == 1
-#pragma unroll
-          for (int k = 0; k < SEG; ++k) box[k] = w[k + H];
-#else
           boxcar_segment<H>(w, box);
-#endif
           if (segment_interior(bin0, n, half)) {
             scaled = !a.dense_box;
             if (!scaled) {
@@ -763,7 +649,6 @@ __global__ void __maxnreg__(kDetectRegs) k_detect(const DetectArgs a, const __gr
         }
       }
       if (!released && tile + kAvgBuffers < n_tiles) bar_arrive(kBarEmpty + sb, kSumThreads + kBoxThreads);  // this average buffer may be overwritten
-      const long long b2c = btr ? clock64() : 0;
       constexpr int XD = HALF_T > 0 ? 2 * HALF_T + 1 : 1;
       auto value_of = [&](float b) { return scaled ? div_const_fast<XD>(b) : b; };  // average(avg, X)[bin], utils.cpp:49
       const float lvl_detect = scaled ? a.detect_sum : a.detect_level, lvl_start = scaled ? a.start_sum : a.start_level;
@@ -850,14 +735,7 @@ __global__ void __maxnreg__(kDetectRegs) k_detect(const DetectArgs a, const __gr
           ++pos;
         }
       }
-      if (btr) {
-        const long long b3c = clock64();
-        btr_c[0] += b1c - b0c;
-        btr_c[1] += b2c - b1c;
-        btr_c[2] += b3c - b2c;
-      }
     }
-    if (btr) printf("[k_detect cta %d] box warp g0 s%d: wait FULL %lld, load+div+boxcar %lld, entries+rest %lld\n", blockIdx.x, seg, btr_c[0], btr_c[1], btr_c[2]);
     if (a.cta_ns && btid == 0 && group == (n_tiles - 1) % kBoxGroups) a.cta_ns[2 * blockIdx.x + 1] = global_timer_ns();
   }
 }

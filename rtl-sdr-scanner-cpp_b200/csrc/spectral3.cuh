@@ -81,32 +81,15 @@ __device__ __forceinline__ void dft32(C* v) {
   }
 }
 
-// Complex value type of k_spectrum3: cpk = every half an explicitly rounded scalar operation, in the rounding order that
-// defines this kernel's results (b2s_device.cuh); float2 = the contractible helpers (A/B builds: -DB2S_K1_PACKED=0, results
-// differ in the last bits).
-#ifndef B2S_K1_PACKED
-#define B2S_K1_PACKED 1
-#endif
-// A/B switches (all three on by default):
-//   B2S_K1_PAIR_A      (RA < 16 only) pass A handles two ADJACENT columns per thread step: 4-byte sample loads, 8-byte window
-//                      loads, 16-byte twiddle loads and 16-byte exchange stores instead of twice as many half-width ones
-//   B2S_K1_DEFER_OUT   the dB row is gathered into registers, the block barrier follows at once, and the global stores (+ the
-//                      first-maximum search) are issued behind it, beside the next frame's pass A
-//   B2S_K1_LOAD_ORDER  passes B and C load their 32 inputs in the order the first radix-4 butterflies consume them
-#ifndef B2S_K1_PAIR_A
-#define B2S_K1_PAIR_A 1
-#endif
-#ifndef B2S_K1_DEFER_OUT
-#define B2S_K1_DEFER_OUT 1
-#endif
-#ifndef B2S_K1_LOAD_ORDER
-#define B2S_K1_LOAD_ORDER 1
-#endif
-#if B2S_K1_PACKED
-using K1Complex = cpk;
-#else
-using K1Complex = float2;
-#endif
+// The complex values of k_spectrum3 are cpk: every half an explicitly rounded scalar operation, in the rounding order that
+// defines this kernel's results (b2s_device.cuh).
+//
+// Two code paths are chosen by the transform size:
+//   kPairA (RA < 16)  pass A handles two ADJACENT columns per thread step: 4-byte sample loads, 8-byte window loads, 16-byte
+//                     twiddle loads and 16-byte exchange stores instead of twice as many half-width ones
+//   kDefer (!SPLIT)   the dB row is gathered into registers, the block barrier follows at once, and the global stores (+ the
+//                     first-maximum search) are issued behind it, beside the next frame's pass A
+// Passes B and C load their 32 inputs in the order the first radix-4 butterflies consume them.
 
 constexpr int kBlockPitch = 32 * 33;  // float2 elements per warp-owned block (32 rows of pitch 33 after pass B)
 
@@ -144,7 +127,7 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
   static_assert(!SPLIT || RA == 16, "the split mode runs 16384-point sub-transforms");
   static_assert(SPLIT_S == 1 || SPLIT_S == 2 || SPLIT_S == 4 || SPLIT_S == 8 || SPLIT_S == 16, "S");
   extern __shared__ __align__(128) unsigned char smem[];
-  using C = K1Complex;
+  using C = cpk;
   C* X = reinterpret_cast<C*>(smem);                                           // [RA][kBlockPitch]
   float2* twB = reinterpret_cast<float2*>(X + RA * kBlockPitch);               // [31][32]
   unsigned char* raw = reinterpret_cast<unsigned char*>(twB + 31 * 32);        // TMA mode: 2M bytes, or 2 x kSplitStageBytes (split)
@@ -190,8 +173,8 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
     if (SPLIT) issue(item, 1, 1);
   }
 
-  constexpr bool kDefer = B2S_K1_DEFER_OUT && !SPLIT;
-  constexpr bool kPairA = B2S_K1_PAIR_A && RA < 16;  // pairing helps where several CTAs share an SM (N <= 8192)
+  constexpr bool kDefer = !SPLIT;
+  constexpr bool kPairA = RA < 16;  // pairing helps where several CTAs share an SM (N <= 8192)
   int pend_frame = -1;   // kDefer: frame whose first maximum is still being collected in red_i[(round - 1) & 1]
   float pend_max = 0.0f;
   uint32_t parity = 0;   // non-split: phase of full_bar[0]
@@ -338,32 +321,22 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
     // ---------------- passes B and C: warp `warp` owns block k0 = warp ----------------
     C v[32];
     C* blk = X + warp * kBlockPitch;
-#if B2S_K1_LOAD_ORDER
 #pragma unroll
-    for (int q = 0; q < 32; ++q) {  // in the order dft32's radix-4 butterflies take them: (n2 = 0: 0 8 16 24), (n2 = 1: 1 9 17 25), ...
+    for (int q = 0; q < 32; ++q) {  // element (n1 = m, n2 = lane), in the order dft32's radix-4 butterflies take them: (n2 = 0: 0 8 16 24), (n2 = 1: 1 9 17 25), ...
       const int m = 8 * (q & 3) + (q >> 2);
       v[m] = blk[m * 32 + lane];
     }
-#else
-#pragma unroll
-    for (int m = 0; m < 32; ++m) v[m] = blk[m * 32 + lane];  // element (n1 = m, n2 = lane)
-#endif
     __syncwarp();                                             // every lane has its inputs before anyone overwrites the block
     dft32(v);
     blk[lane * 33] = v[0];
 #pragma unroll
     for (int k1 = 1; k1 < 32; ++k1) blk[lane * 33 + k1] = cmul(v[k1], twB[(k1 - 1) * 32 + lane]);  // transposed: [n2][k1], pitch 33
     __syncwarp();
-#if B2S_K1_LOAD_ORDER
 #pragma unroll
-    for (int q = 0; q < 32; ++q) {
+    for (int q = 0; q < 32; ++q) {  // element (k1 = lane, n2 = m), same order
       const int m = 8 * (q & 3) + (q >> 2);
       v[m] = blk[m * 33 + lane];
     }
-#else
-#pragma unroll
-    for (int m = 0; m < 32; ++m) v[m] = blk[m * 33 + lane];  // element (k1 = lane, n2 = m)
-#endif
     __syncwarp();
     dft32(v);
     // lane k1 holds X[k0 + RA*k1 + 32*RA*k2] in v[k2]: |X|^2/fs -> dB (psd.cpp:18), parked in the warp's block as [k2][k1]

@@ -54,8 +54,6 @@ struct TrackResult {  // what the host reads back per push
   int n_tx, n_entries, max_count, error;
   long long last_now;
   int n_evals, n_events, n_best, pad;  // work counters of the push: block evaluations, event frames replayed, getBestIndex calls
-  long long cycles;                    // SM cycles k_track ran
-  long long phase[4];                  // of which: folding entries into runs, evaluations, event walks (commits + event frames), output
   b2s_transmission tx[kMaxSignals];  // getSortedTransmissions after the last frame
 };
 
@@ -79,7 +77,6 @@ struct TrackArgs {
   const float* ring_before;    // [Y][N] ring before the push, oldest -> newest
   TrackState* state;
   TrackResult* result;
-  int debug;  // printf trace of the evaluations and event frames (B2S_TRACK_DEBUG=2)
 };
 
 __device__ __forceinline__ long long track_frame_time(long long t0, double period, long long k) {
@@ -212,14 +209,7 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track(const TrackArgs a) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int T = a.n_frames;
   const int gh = p.group_size / 2, margin = track_margin(p.group_size);
-  const long long clock_begin = clock64();
   int n_evals = 0, n_events = 0, n_best = 0;  // (thread 0's copies are reported)
-  long long ph[4] = {0, 0, 0, 0}, ph_t = clock_begin;
-  auto lap = [&](int i) {
-    const long long c = clock64();
-    ph[i] += c - ph_t;
-    ph_t = c;
-  };
 
   // ---- load the map ----
   if (tid == 0) {
@@ -263,7 +253,6 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track(const TrackArgs a) {
     const long long now = s.time[tid];
     const bool complex_frame = n_stop > kRunCap || n_start > kRunCap;  // replayed from its raw entries
     __syncthreads();
-    lap(0);
     int ts = bs;  // first frame of the block not yet applied (uniform)
     while (ts < be) {
       // ================= evaluation: events of the frames [ts, be) under the current key set =================
@@ -322,12 +311,6 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track(const TrackArgs a) {
       }
       if (tid == 0) s.changed = 0;
       __syncthreads();
-      lap(1);
-      if (a.debug && tid == 0) {
-        printf("[k_track] eval ts=%d be=%d K=%d evmask %08x %08x hit0 %08x %08x", ts, be, K, s.evmask[0], s.evmask[1], K > 0 ? s.hit[0][0] : 0u, K > 0 ? s.hit[0][1] : 0u);
-        for (int q = 0; q < K; ++q) printf(" key%d last %lld", s.key[q], s.last[q]);
-        printf("\n");
-      }
       // ================= walk the event frames in order until one of them changes the key set =================
       int cur = ts;
       while (true) {
@@ -355,7 +338,6 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track(const TrackArgs a) {
         }
         // ---- the event frame te, exactly as Transmission::process orders it (transmission.cpp:57-68) ----
         ++n_events;
-        if (a.debug && tid == 0) printf("[k_track]   event frame %d (cur %d)\n", te, cur);
         const long long ev_now = s.time[te - bs];
         const int e0 = a.offsets[te], e1 = a.offsets[te + 1];
         if (tid == 0) {
@@ -464,7 +446,6 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track(const TrackArgs a) {
         }
       }
       __syncthreads();
-      lap(2);
     }
   }
 
@@ -511,9 +492,6 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track(const TrackArgs a) {
     a.result->n_evals = n_evals;
     a.result->n_events = n_events;
     a.result->n_best = n_best;
-    lap(3);
-    a.result->cycles = clock64() - clock_begin;
-    for (int i = 0; i < 4; ++i) a.result->phase[i] = ph[i];
   }
 }
 
