@@ -292,6 +292,32 @@ int b2s_pack_spectrogram_message(int64_t time_ms, int32_t center_hz, int32_t sam
 int b2s_pack_transmission_message(int64_t time_ms, int32_t frequency_hz, int32_t sample_rate_hz, const int8_t* iq, int n_samples, uint8_t* out,
                                   size_t cap, size_t* written); /* DataController::pushTransmission, data_controller.cpp:27-42 */
 
+/* ---- recorder bank: a device's pool of Recorders on one IQ stream (SdrDevice::m_recorders, sdr_device.cpp:39-41,82-144) ----
+ * n_channels recorders that share one source, indexed like the scan policy's b2s_recorder_action.recorder. A channel computes exactly
+ * the bytes of a b2s_recorder with the same rate, bandwidth, format and scale, started with the same shift before the same push and
+ * fed the same pushes, whatever the other channels do. One push runs every recording channel: at most one host-to-device copy, one
+ * launch per stage (per 64 recording channels), one device-to-host copy and one synchronise.
+ * Like Recorder (recorder.cpp:35-39, buffer.h:22-55) each channel cuts its int8 output into chunks of
+ * chunk_samples = roundUp(bandwidth * 100 / 1000, 4096) samples; chunk j (from 0) of a recording is stamped
+ * start_ms + floor((j + 1) * chunk_samples * 1000 / bandwidth + 0.5), start_ms = t0_ms of the first non-empty push after start.
+ * A push that would not fit (n_samples > max_samples_per_push, or an output longer than cap_samples) returns B2S_E_INVALID
+ * before any work and changes nothing. */
+typedef struct b2s_recorder_bank b2s_recorder_bank;
+int b2s_recorder_bank_create(b2s_engine* e, int32_t sample_rate_hz, int32_t bandwidth_hz, int iq_format, float iq_scale,
+                             int flags /* B2S_FLAG_IQ_ON_DEVICE */, int n_channels, size_t max_samples_per_push /* 0 -> 4 Mi */,
+                             b2s_recorder_bank** out);
+int b2s_recorder_bank_destroy(b2s_recorder_bank* k);
+int b2s_recorder_bank_start(b2s_recorder_bank* k, int channel, int32_t shift_hz); /* Recorder::startRecording; B2S_E_STATE when recording */
+int b2s_recorder_bank_stop(b2s_recorder_bank* k, int channel);                    /* Recorder::stopRecording: discards buffered output; B2S_E_STATE when idle */
+/* the stream's next n_samples (t0_ms = injected time of the first one) through every recording channel.
+   out_iq: optional [n_channels][cap_samples] int8 pairs (host); n_out: optional [n_channels] (0 for idle channels) */
+int b2s_recorder_bank_push(b2s_recorder_bank* k, const void* iq, size_t n_samples, int64_t t0_ms,
+                           int8_t* out_iq, size_t cap_samples, size_t* n_out);
+/* Recorder::flush: the complete chunks buffered since the last flush, oldest first; up to `cap` are copied, *count = chunks available;
+   with consume != 0 the chunks copied out (and only those) are dropped */
+int b2s_recorder_bank_flush(b2s_recorder_bank* k, int channel, int8_t* chunks /*[cap][chunk_samples][2]*/, int64_t* times_ms,
+                            int cap, int consume, int* count, int* chunk_samples);
+
 #ifdef __cplusplus
 }
 #endif

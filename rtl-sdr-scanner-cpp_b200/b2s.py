@@ -633,6 +633,68 @@ class Recorder:
             pass
 
 
+class RecorderBank:
+    """A device's pool of Recorders on one IQ stream (SdrDevice::m_recorders, sdr_device.cpp:39-41): n_channels recorders indexed like
+    the scan policy's actions. Each push runs every recording channel; each channel keeps Recorder's timestamped chunks for flush()."""
+
+    def __init__(self, engine: Engine, sample_rate_hz: int, bandwidth_hz: int, n_channels: int, iq_format: int = IQ_CS8, iq_scale: float = 1.0 / 127.0,
+                 on_device: bool = False, max_samples_per_push: int = 0):
+        L = lib()
+        L.b2s_recorder_bank_create.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int, C.c_float, C.c_int, C.c_int, C.c_size_t, C.POINTER(C.c_void_p)]
+        L.b2s_recorder_bank_destroy.argtypes = [C.c_void_p]
+        L.b2s_recorder_bank_start.argtypes = [C.c_void_p, C.c_int, C.c_int32]
+        L.b2s_recorder_bank_stop.argtypes = [C.c_void_p, C.c_int]
+        L.b2s_recorder_bank_push.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]
+        L.b2s_recorder_bank_flush.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+        self._e = engine
+        self.sample_rate_hz, self.bandwidth_hz, self.n_channels, self.iq_format = sample_rate_hz, bandwidth_hz, n_channels, iq_format
+        self._h = C.c_void_p()
+        _check(L.b2s_recorder_bank_create(engine._h, sample_rate_hz, bandwidth_hz, iq_format, iq_scale, FLAG_IQ_ON_DEVICE if on_device else 0, n_channels,
+                                          max_samples_per_push, C.byref(self._h)))
+
+    def start(self, channel: int, shift_hz: int):
+        _check(lib().b2s_recorder_bank_start(self._h, channel, shift_hz))
+
+    def stop(self, channel: int):
+        _check(lib().b2s_recorder_bank_stop(self._h, channel))
+
+    def push(self, iq, t0_ms: int = 0, n_samples: int = None):
+        """iq: numpy array of the stream's next samples (int8 pairs or float32 pairs), or a raw device pointer with n_samples.
+        Returns one int8 pair array per channel (empty for idle channels)."""
+        if isinstance(iq, np.ndarray):
+            iq = np.ascontiguousarray(iq)
+            n_samples = iq.size // 2
+            ptr = _ptr(iq)
+        else:
+            ptr = C.c_void_p(iq)
+        cap = n_samples * self.bandwidth_hz // self.sample_rate_hz + 64
+        out = np.empty((self.n_channels, 2 * cap), np.int8)
+        n_out = np.zeros(self.n_channels, np.uint64)
+        _check(lib().b2s_recorder_bank_push(self._h, ptr, n_samples, int(t0_ms), _ptr(out), cap, _ptr(n_out)))
+        return [out[c, : 2 * int(n_out[c])] for c in range(self.n_channels)]
+
+    def flush(self, channel: int, cap: int = 256, consume: bool = True):
+        """Recorder::flush: [(time_ms, int8 pairs of one chunk)] for the complete chunks buffered since the last flush, oldest first."""
+        count, cs = C.c_int(), C.c_int()
+        _check(lib().b2s_recorder_bank_flush(self._h, channel, None, None, 0, 0, C.byref(count), C.byref(cs)))
+        k = min(count.value, cap)
+        chunks = np.empty((k, 2 * cs.value), np.int8)
+        times = np.empty(k, np.int64)
+        _check(lib().b2s_recorder_bank_flush(self._h, channel, _ptr(chunks), _ptr(times), k, 1 if consume else 0, C.byref(count), C.byref(cs)))
+        return [(int(times[i]), chunks[i]) for i in range(k)]
+
+    def close(self):
+        if self._h:
+            lib().b2s_recorder_bank_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class RecorderAction(C.Structure):
     _fields_ = [("kind", C.c_int32), ("recorder", C.c_int32), ("shift_hz", C.c_int32), ("duration_ms", C.c_int64)]
 

@@ -13,6 +13,11 @@
 // int8 / float IQ and applies the rotation while it fills the tile (phase from a 64-bit fixed-point accumulator: exact to 2^-65
 // turns per sample, so no drift however long the recording), the last stage packs to int8 (round to nearest even, saturate:
 // volk_32f_s32f_convert_8i).
+//
+// A launch serves up to kLaunchChannels recording channels of a recorder bank (SdrDevice's pool of Recorders on one source,
+// sdr_device.cpp:39-41): every channel runs the same stages on the same stream, each with its own shift, start and buffers. CTA b
+// works for channel b % n_ch, so the CTAs of all channels that cover the same span of the stream are adjacent in launch order. In
+// the first stage they read the same raw samples: one read from HBM, the others from L2. A stand-alone recorder is a bank of one.
 #pragma once
 #include <cmath>
 #include <vector>
@@ -23,26 +28,50 @@ namespace b2s {
 
 constexpr int kResampleThreads = 128;
 constexpr int kResampleTile = 6000;  // input samples held in shared memory per CTA (48 KB of float2)
+constexpr int kLaunchChannels = 64;  // channels per stage launch (their geometry travels in the kernel parameters)
 
-struct ResampleArgs {
-  // input of this launch: `n_in` new samples `in` (global sample index g0 ...), preceded by `hc` carried samples in `carry`
-  const void* in;
-  const void* carry;
-  int kind;        // 0: int8 pairs, 1: float pairs (raw IQ); 2: float2 (output of the previous stage)
-  float iq_scale;  // int8 only
-  long long g0;
-  int n_in, hc;
+// one channel's part of a stage launch; indices count from the channel's startRecording
+struct StageChan {
+  long long g0;                  // index of the first new input sample
+  long long m0;                  // index of the first output of this launch
   unsigned long long phase_inc;  // rotation per input sample in turns * 2^64 (first stage; 0 = none)
-  const float* taps;
-  int n_taps, interp, decim;
-  long long m0;  // global index of the first output of this launch
-  int n_out, per_cta;
-  float2* out_f;         // next stage's input, or ...
-  signed char* out_i8;   // ... the int8 pairs of the last stage
+  int n_in, n_out;
+  int slot;                      // the channel's row in the per-channel buffers
 };
 
+struct ResampleArgs {
+  // input of this launch, per channel: `n_in` new samples at `in`, preceded by `hc` carried samples at `carry`, both offset by
+  // slot * in_stride elements (0 for the raw stream, which every channel shares)
+  const void* in;
+  const void* carry;
+  long long in_stride;
+  int kind;        // 0: int8 pairs, 1: float pairs (raw IQ); 2: float2 (output of the previous stage)
+  float iq_scale;  // int8 only
+  int hc;
+  const float* taps;
+  int n_taps, interp, decim, per_cta;
+  float2* out_f;         // next stage's input, or ...
+  signed char* out_i8;   // ... the int8 pairs of the last stage; row `slot` starts at slot * out_stride samples
+  long long out_stride;
+  int n_ch;
+  StageChan ch[kLaunchChannels];
+};
+
+// what one CTA reads: its channel's view of the stage input
+struct StageView {
+  const void* in;
+  const void* carry;
+  long long g0;
+  int n_in, hc, kind;
+  float iq_scale;
+};
+__device__ __forceinline__ StageView stage_view(const ResampleArgs& a, const StageChan& c) {
+  const long long off = static_cast<long long>(c.slot) * a.in_stride * (a.kind == 0 ? 2 : 8);
+  return StageView{static_cast<const char*>(a.in) + off, static_cast<const char*>(a.carry) + off, c.g0, c.n_in, a.hc, a.kind, a.iq_scale};
+}
+
 // sample g of this stage's input stream, before the rotator (zero before startRecording)
-__device__ __forceinline__ float2 resample_raw(const ResampleArgs& a, long long g) {
+__device__ __forceinline__ float2 resample_raw(const StageView& a, long long g) {
   if (g < 0) return make_float2(0.0f, 0.0f);
   const long long rel = g - a.g0;
   if (rel >= a.n_in) return make_float2(0.0f, 0.0f);  // past the newest sample (the last CTA of k_decimate_poly stages a whole tile; only unused outputs see these)
@@ -61,12 +90,12 @@ __device__ __forceinline__ float2 rotor_of(unsigned long long turns64) {
   return make_float2(cs, sn);
 }
 
-__device__ __forceinline__ float2 resample_input(const ResampleArgs& a, long long g) {
+__device__ __forceinline__ float2 resample_input(const StageView& a, unsigned long long phase_inc, long long g) {
   if (g < 0) return make_float2(0.0f, 0.0f);  // before startRecording: zero history
   float2 v = resample_raw(a, g);
   if (a.kind == 2) return v;
-  if (a.phase_inc) {  // rotator_cc: x[n] * exp(i * phase_inc * n)
-    const unsigned long long ph = static_cast<unsigned long long>(g) * a.phase_inc;  // turns * 2^64, modulo 1 turn by overflow
+  if (phase_inc) {  // rotator_cc: x[n] * exp(i * phase_inc * n)
+    const unsigned long long ph = static_cast<unsigned long long>(g) * phase_inc;  // turns * 2^64, modulo 1 turn by overflow
     float sn, cs;
     sincospif(static_cast<float>(static_cast<unsigned int>(ph >> 32)) * (2.0f / 4294967296.0f), &sn, &cs);
     v = make_float2(fmaf(v.x, cs, -v.y * sn), fmaf(v.x, sn, v.y * cs));
@@ -74,17 +103,20 @@ __device__ __forceinline__ float2 resample_input(const ResampleArgs& a, long lon
   return v;
 }
 
-__global__ void __launch_bounds__(kResampleThreads) k_resample(const ResampleArgs a) {
+__global__ void __launch_bounds__(kResampleThreads) k_resample(const __grid_constant__ ResampleArgs a) {
   extern __shared__ float2 tile[];
   const int tid = threadIdx.x;
-  const long long mb = a.m0 + static_cast<long long>(blockIdx.x) * a.per_cta;  // first output of this CTA
-  const int count = min(a.per_cta, a.n_out - blockIdx.x * a.per_cta);
+  const StageChan& c = a.ch[blockIdx.x % a.n_ch];
+  const int cta = blockIdx.x / a.n_ch;
+  const StageView v = stage_view(a, c);
+  const long long mb = c.m0 + static_cast<long long>(cta) * a.per_cta;  // first output of this CTA
+  const int count = min(a.per_cta, c.n_out - cta * a.per_cta);
   if (count <= 0) return;
   // inputs needed: u indices [mb D - (n_taps - 1), (mb + count - 1) D]  ->  x indices [floor(lo / I) .. floor(hi / I)]
   const long long u_lo = mb * a.decim - (a.n_taps - 1), u_hi = (mb + count - 1) * a.decim;
   const long long x_lo = u_lo >= 0 ? u_lo / a.interp : -((-u_lo + a.interp - 1) / a.interp), x_hi = u_hi / a.interp;
   const int span = static_cast<int>(x_hi - x_lo + 1);
-  for (int i = tid; i < span; i += kResampleThreads) tile[i] = resample_input(a, x_lo + i);
+  for (int i = tid; i < span; i += kResampleThreads) tile[i] = resample_input(v, c.phase_inc, x_lo + i);
   __syncthreads();
   for (int o = tid; o < count; o += kResampleThreads) {
     const long long m = mb + o;
@@ -99,7 +131,7 @@ __global__ void __launch_bounds__(kResampleThreads) k_resample(const ResampleArg
       re = fmaf(h, v.x, re);
       im = fmaf(h, v.y, im);
     }
-    const long long oi = m - a.m0;
+    const long long oi = c.slot * a.out_stride + (m - c.m0);
     if (a.out_i8) {  // complex_to_interleaved_char(vector, 127): rint, saturate
       const int r = max(-128, min(127, __float2int_rn(re * 127.0f))), q = max(-128, min(127, __float2int_rn(im * 127.0f)));
       a.out_i8[2 * oi] = static_cast<signed char>(r);
@@ -124,22 +156,26 @@ constexpr int kPolyThreads = 128;
 constexpr int kPolyOut = kPolyThreads * kPolyR;   // outputs per CTA
 constexpr int kPolyTile = kPolyOut + kPolyQ - 1;  // samples of one phase a CTA needs
 
-__global__ void __launch_bounds__(kPolyThreads) k_decimate_poly(const ResampleArgs a, const float* __restrict__ taps_pq /* [D][kPolyQ]: h[q D + p], zero padded */) {
+__global__ void __launch_bounds__(kPolyThreads) k_decimate_poly(const __grid_constant__ ResampleArgs a, const float* __restrict__ taps_pq /* [D][kPolyQ]: h[q D + p], zero padded */) {
   __shared__ float2 tile[2][kPolyTile];
   __shared__ float htap[2][kPolyQ];
   const int tid = threadIdx.x;
   const int D = a.decim;
-  const long long mb = a.m0 + static_cast<long long>(blockIdx.x) * kPolyOut;  // first output of this CTA
-  const int count = min(kPolyOut, a.n_out - static_cast<int>(blockIdx.x) * kPolyOut);
+  const StageChan& c = a.ch[blockIdx.x % a.n_ch];
+  const int cta = blockIdx.x / a.n_ch;
+  const StageView sv = stage_view(a, c);
+  const long long mb = c.m0 + static_cast<long long>(cta) * kPolyOut;  // first output of this CTA
+  const int count = min(kPolyOut, c.n_out - cta * kPolyOut);
   if (count <= 0) return;
-  const bool rotate = a.kind != 2 && a.phase_inc != 0;
+  const unsigned long long phase_inc = c.phase_inc;
+  const bool rotate = a.kind != 2 && phase_inc != 0;
   // rotor of kPolyThreads tile steps = kPolyThreads * D input samples
-  const float2 rstep = rotate ? rotor_of(static_cast<unsigned long long>(kPolyThreads) * static_cast<unsigned long long>(D) * a.phase_inc) : make_float2(1.0f, 0.0f);
+  const float2 rstep = rotate ? rotor_of(static_cast<unsigned long long>(kPolyThreads) * static_cast<unsigned long long>(D) * phase_inc) : make_float2(1.0f, 0.0f);
   auto fill = [&](int p, int buf) {
     long long g = (mb - (kPolyQ - 1) + tid) * D - p;  // input sample under tile element n = tid
-    float2 r = rotate ? rotor_of(static_cast<unsigned long long>(g) * a.phase_inc) : make_float2(1.0f, 0.0f);
+    float2 r = rotate ? rotor_of(static_cast<unsigned long long>(g) * phase_inc) : make_float2(1.0f, 0.0f);
     for (int n = tid; n < kPolyTile; n += kPolyThreads, g += static_cast<long long>(kPolyThreads) * D) {
-      float2 v = resample_raw(a, g);
+      float2 v = resample_raw(sv, g);
       if (rotate) {
         v = make_float2(fmaf(v.x, r.x, -v.y * r.y), fmaf(v.x, r.y, v.y * r.x));
         r = make_float2(fmaf(r.x, rstep.x, -r.y * rstep.y), fmaf(r.x, rstep.y, r.y * rstep.x));
@@ -175,7 +211,7 @@ __global__ void __launch_bounds__(kPolyThreads) k_decimate_poly(const ResampleAr
   for (int r = 0; r < kPolyR; ++r) {
     const int o = tid * kPolyR + r;
     if (o < count) {
-      const long long oi = mb + o - a.m0;
+      const long long oi = c.slot * a.out_stride + (mb + o - c.m0);
       if (a.out_i8) {  // complex_to_interleaved_char(vector, 127): rint, saturate
         const int re = max(-128, min(127, __float2int_rn(acc[r].x * 127.0f))), im = max(-128, min(127, __float2int_rn(acc[r].y * 127.0f)));
         reinterpret_cast<char2*>(a.out_i8)[oi] = make_char2(static_cast<signed char>(re), static_cast<signed char>(im));
