@@ -238,21 +238,16 @@ def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
-class Engine:
-    """b2s_engine: one per GPU (reference analogue: the process that owns the SdrDevice chains)."""
+class _Handle:
+    """Owns one C-ABI handle `_h`: close() (or garbage collection) passes it to its b2s_*_destroy function once."""
 
-    def __init__(self, cuda_device: int = 0):
+    def __init__(self, destroy):
         self._h = C.c_void_p()
-        _check(lib().b2s_engine_create(cuda_device, C.byref(self._h)))
-
-    def device_name(self) -> str:
-        buf = C.create_string_buffer(256)
-        _check(lib().b2s_engine_device_name(self._h, buf, 256))
-        return buf.value.decode()
+        self._destroy = destroy
 
     def close(self):
         if self._h:
-            lib().b2s_engine_destroy(self._h)
+            self._destroy(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):
@@ -260,6 +255,19 @@ class Engine:
             self.close()
         except Exception:
             pass
+
+
+class Engine(_Handle):
+    """b2s_engine: one per GPU (reference analogue: the process that owns the SdrDevice chains)."""
+
+    def __init__(self, cuda_device: int = 0):
+        super().__init__(lib().b2s_engine_destroy)
+        _check(lib().b2s_engine_create(cuda_device, C.byref(self._h)))
+
+    def device_name(self) -> str:
+        buf = C.create_string_buffer(256)
+        _check(lib().b2s_engine_device_name(self._h, buf, 256))
+        return buf.value.decode()
 
     def check_div_const(self, divisor: int) -> int:
         """Mismatches of the engine's exact constant division against IEEE division over its whole guarded range (must be 0)."""
@@ -287,13 +295,13 @@ class Engine:
         return (psd, lin) if want_linear else psd
 
 
-class Averager:
+class Averager(_Handle):
     """Device-backed Averager with the reference's surface (sources/radio/averager.h:8-28)."""
 
     def __init__(self, engine: Engine, size: int, group_size: int):
+        super().__init__(lib().b2s_averager_destroy)
         self._e = engine
         self.size, self.group_size = size, group_size
-        self._h = C.c_void_p()
         _check(lib().b2s_averager_create(engine._h, size, group_size, C.byref(self._h)))
 
     def push(self, data):
@@ -323,17 +331,6 @@ class Averager:
         _check(lib().b2s_averager_sum(self._h, _ptr(out), C.byref(frames)))
         return out, frames.value
 
-    def close(self):
-        if self._h:
-            lib().b2s_averager_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 class PushOutput:
     """Host-side view of one b2s_band_push result."""
@@ -348,13 +345,13 @@ class PushOutput:
         self.n_spectrogram_rows = 0
 
 
-class Band:
+class Band(_Handle):
     """b2s_band: the GPU replacement of one device's decimator..transmission(+spectrogram) chain."""
 
     def __init__(self, engine: Engine, cfg: BandConfig):
+        super().__init__(lib().b2s_band_destroy)
         self._e = engine
         self.cfg = cfg
-        self._h = C.c_void_p()
         _check(lib().b2s_band_create(engine._h, C.byref(cfg), C.byref(self._h)))
 
     def set_stream(self, cuda_stream: int):
@@ -467,17 +464,6 @@ class Band:
         k = min(count.value, cap)
         return keys[:k], first[:k], last[:k], power[:k]
 
-    def close(self):
-        if self._h:
-            lib().b2s_band_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 # ---- host helpers (reference semantics) ----
 def get_fft(sample_rate_hz: int, max_step_hz: int) -> int:
@@ -488,13 +474,13 @@ def get_tuned_frequency(f: int, step: int) -> int:
     return lib().b2s_get_tuned_frequency(f, step)
 
 
-class HostTransmission:
+class HostTransmission(_Handle):
     """Transmission bookkeeping on host rows (b2s_host_transmission_*): the band's tracker without the GPU. push() returns,
     per frame, the list of (shift_hz, flush, key, power) exactly as Transmission::getSortedTransmissions orders it."""
 
     def __init__(self, cfg: BandConfig):
+        super().__init__(lib().b2s_host_transmission_destroy)
         self.cfg = cfg
-        self._h = C.c_void_p()
         _check(lib().b2s_host_transmission_create(C.byref(cfg), C.byref(self._h)))
 
     def push(self, box_rows: np.ndarray, q_rows: np.ndarray, t0_ms: int, frame_period_ms: float, use_watch: bool = True):
@@ -514,17 +500,6 @@ class HostTransmission:
 
     def reset(self):
         _check(lib().b2s_host_transmission_reset(self._h))
-
-    def close(self):
-        if self._h:
-            lib().b2s_host_transmission_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def _pack(fn, time_ms: int, frequency_hz: int, sample_rate_hz: int, data: np.ndarray, count: int, header: int) -> bytes:
@@ -572,7 +547,7 @@ def get_resamplers_factors(sample_rate_hz: int, bandwidth_hz: int, threshold: in
     return [(a[i], b[i]) for i in range(k)]
 
 
-class Recorder:
+class Recorder(_Handle):
     """The DSP chain of one reference Recorder on the GPU (recorder.cpp:22-40,58-73): rotate by -shift, resample fs -> bandwidth, int8."""
 
     def __init__(self, engine: Engine, sample_rate_hz: int, bandwidth_hz: int, iq_format: int = IQ_CS8, iq_scale: float = 1.0 / 127.0, on_device: bool = False,
@@ -585,9 +560,9 @@ class Recorder:
         L.b2s_recorder_push.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
         L.b2s_recorder_stages.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         L.b2s_recorder_taps.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
+        super().__init__(L.b2s_recorder_destroy)
         self._e = engine
         self.sample_rate_hz, self.bandwidth_hz, self.iq_format = sample_rate_hz, bandwidth_hz, iq_format
-        self._h = C.c_void_p()
         _check(L.b2s_recorder_create(engine._h, sample_rate_hz, bandwidth_hz, iq_format, iq_scale, FLAG_IQ_ON_DEVICE if on_device else 0, max_samples_per_push, C.byref(self._h)))
 
     def stages(self):
@@ -621,19 +596,8 @@ class Recorder:
         _check(lib().b2s_recorder_push(self._h, ptr, n_samples, _ptr(out), cap, C.byref(n_out)))
         return out[: 2 * n_out.value]
 
-    def close(self):
-        if self._h:
-            lib().b2s_recorder_destroy(self._h)
-            self._h = C.c_void_p()
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class RecorderBank:
+class RecorderBank(_Handle):
     """A device's pool of Recorders on one IQ stream (SdrDevice::m_recorders, sdr_device.cpp:39-41): n_channels recorders indexed like
     the scan policy's actions. Each push runs every recording channel; each channel keeps Recorder's timestamped chunks for flush()."""
 
@@ -646,9 +610,9 @@ class RecorderBank:
         L.b2s_recorder_bank_stop.argtypes = [C.c_void_p, C.c_int]
         L.b2s_recorder_bank_push.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]
         L.b2s_recorder_bank_flush.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+        super().__init__(L.b2s_recorder_bank_destroy)
         self._e = engine
         self.sample_rate_hz, self.bandwidth_hz, self.n_channels, self.iq_format = sample_rate_hz, bandwidth_hz, n_channels, iq_format
-        self._h = C.c_void_p()
         _check(L.b2s_recorder_bank_create(engine._h, sample_rate_hz, bandwidth_hz, iq_format, iq_scale, FLAG_IQ_ON_DEVICE if on_device else 0, n_channels,
                                           max_samples_per_push, C.byref(self._h)))
 
@@ -683,17 +647,6 @@ class RecorderBank:
         _check(lib().b2s_recorder_bank_flush(self._h, channel, _ptr(chunks), _ptr(times), k, 1 if consume else 0, C.byref(count), C.byref(cs)))
         return [(int(times[i]), chunks[i]) for i in range(k)]
 
-    def close(self):
-        if self._h:
-            lib().b2s_recorder_bank_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 class RecorderAction(C.Structure):
     _fields_ = [("kind", C.c_int32), ("recorder", C.c_int32), ("shift_hz", C.c_int32), ("duration_ms", C.c_int64)]
@@ -707,7 +660,7 @@ def get_range_split_sample_rate(sample_rate_hz: int) -> int:
     return lib().b2s_get_range_split_sample_rate(sample_rate_hz)
 
 
-class ScanPolicy:
+class ScanPolicy(_Handle):
     """Scanner's hop rule (scanner.cpp:36-64) and SdrDevice::updateRecordings (sdr_device.cpp:82-144) as a host state machine."""
 
     def __init__(self, ranges, sample_rate_hz: int, n_recorders: int, scanning_time_ms: int = 500):
@@ -719,7 +672,7 @@ class ScanPolicy:
         L.b2s_scan_policy_notify.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
         lo = np.array([r[0] for r in ranges], np.int32)
         hi = np.array([r[1] for r in ranges], np.int32)
-        self._h = C.c_void_p()
+        super().__init__(L.b2s_scan_policy_destroy)
         _check(L.b2s_scan_policy_create(_ptr(lo), _ptr(hi), len(ranges), sample_rate_hz, n_recorders, scanning_time_ms, C.byref(self._h)))
 
     def ranges(self):
@@ -743,14 +696,3 @@ class ScanPolicy:
         _check(lib().b2s_scan_policy_notify(self._h, now_ms, C.cast(tx, C.c_void_p), n, C.cast(acts, C.c_void_p), 256, C.byref(na), C.byref(hop), C.byref(lo), C.byref(hi)))
         out = [(acts[i].kind, acts[i].recorder, acts[i].shift_hz, acts[i].duration_ms) for i in range(min(na.value, 256))]
         return out, ((lo.value, hi.value) if hop.value else None)
-
-    def close(self):
-        if self._h:
-            lib().b2s_scan_policy_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass

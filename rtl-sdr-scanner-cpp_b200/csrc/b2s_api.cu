@@ -13,9 +13,12 @@
 #include <deque>
 #include <limits>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <set>
 #include <string>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../include/b2s.h"
@@ -47,45 +50,71 @@ int fail(int code, const char* fmt, ...) {
     if (err__ != cudaSuccess) return fail(B2S_E_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(err__), __FILE__, __LINE__); \
   } while (0)
 
-template <typename T>
-struct DevBuf {
-  T* p = nullptr;
-  size_t n = 0;
-  int alloc(size_t count) {
-    if (count <= n) return 0;
-    if (p) cudaFree(p);
-    p = nullptr;
-    n = 0;
-    if (cudaMalloc(&p, count * sizeof(T)) != cudaSuccess) return fail(B2S_E_NOMEM, "cudaMalloc of %zu bytes failed", count * sizeof(T));
-    n = count;
-    return 0;
-  }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    n = 0;
-  }
-};
+// The owners of the library's CUDA resources. Each frees what it holds when it is destroyed and can be moved but not copied, so an
+// object's resources go with the object and an early return frees what a function had allocated.
 
-template <typename T>
-struct PinBuf {
+// `count` elements of device memory (DevBuf) or pinned host memory (PinBuf)
+template <typename T, bool kPinned>
+struct CudaBuf {
   T* p = nullptr;
   size_t n = 0;
+  CudaBuf() = default;
+  CudaBuf(CudaBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), n(std::exchange(o.n, 0)) {}
+  CudaBuf& operator=(CudaBuf&& o) noexcept {
+    std::swap(p, o.p);
+    std::swap(n, o.n);
+    return *this;
+  }
+  ~CudaBuf() { free(); }
+  // grow-only; a reallocation does not keep the contents
   int alloc(size_t count) {
     if (count <= n) return 0;
-    if (p) cudaFreeHost(p);
-    p = nullptr;
-    n = 0;
-    if (cudaMallocHost(&p, count * sizeof(T)) != cudaSuccess) return fail(B2S_E_NOMEM, "cudaMallocHost of %zu bytes failed", count * sizeof(T));
+    free();
+    const size_t bytes = count * sizeof(T);
+    if ((kPinned ? cudaMallocHost(&p, bytes) : cudaMalloc(&p, bytes)) != cudaSuccess)
+      return fail(B2S_E_NOMEM, "%s of %zu bytes failed", kPinned ? "cudaMallocHost" : "cudaMalloc", bytes);
     n = count;
     return 0;
   }
-  void release() {
-    if (p) cudaFreeHost(p);
+
+ private:
+  void free() {
+    if (p && kPinned) cudaFreeHost(p);
+    if (p && !kPinned) cudaFree(p);
     p = nullptr;
     n = 0;
   }
 };
+template <typename T>
+using DevBuf = CudaBuf<T, false>;
+template <typename T>
+using PinBuf = CudaBuf<T, true>;
+static_assert(!std::is_copy_constructible<DevBuf<float>>::value && !std::is_copy_assignable<DevBuf<float>>::value, "DevBuf owns its memory");
+static_assert(!std::is_copy_constructible<PinBuf<float>>::value && !std::is_copy_assignable<PinBuf<float>>::value, "PinBuf owns its memory");
+
+// a stream or an event; it is created into `h` by the cudaStreamCreate* / cudaEventCreate* call (and flags) its owner needs
+template <typename H>
+struct CudaHandle {
+  H h = nullptr;
+  CudaHandle() = default;
+  CudaHandle(CudaHandle&& o) noexcept : h(std::exchange(o.h, nullptr)) {}
+  CudaHandle& operator=(CudaHandle&& o) noexcept {
+    std::swap(h, o.h);
+    return *this;
+  }
+  ~CudaHandle() {
+    if (h) destroy(h);
+  }
+  operator H() const { return h; }
+
+ private:
+  static void destroy(cudaStream_t s) { cudaStreamDestroy(s); }
+  static void destroy(cudaEvent_t e) { cudaEventDestroy(e); }
+};
+using Stream = CudaHandle<cudaStream_t>;
+using Event = CudaHandle<cudaEvent_t>;
+static_assert(!std::is_copy_constructible<Stream>::value && !std::is_copy_assignable<Stream>::value, "Stream owns its stream");
+static_assert(!std::is_copy_constructible<Event>::value && !std::is_copy_assignable<Event>::value, "Event owns its event");
 
 bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
@@ -312,13 +341,6 @@ struct SpectralTables {
     sa.split_tw = split_tw.p;
     sa.split_ws = split_ws.p;
   }
-  void release() {
-    wscale.release();
-    twiddle.release();
-    split_tw.release();
-    split_ws.release();
-    work_counter.release();
-  }
 };
 
 int validate_config(const b2s_band_config& c) {
@@ -422,7 +444,7 @@ struct b2s_recorder_bank {
   size_t max_in = 0;
   int n_ch = 0;
   int chunk_samples = 0;  // roundUp(bandwidth * RECORDER_FLUSH_INTERVAL / 1000, 4096), recorder.cpp:35
-  cudaStream_t stream = nullptr;
+  Stream stream;  // declared before the buffers, so it is destroyed after them
   struct Stage {
     int interp = 1, decim = 1, n_taps = 0, hc = 0;
     std::vector<float> h_taps;
@@ -464,25 +486,12 @@ struct b2s_recorder_bank {
     }
   };
   std::vector<Channel> ch;
-  ~b2s_recorder_bank() {
-    for (auto& st : stages) {
-      st.taps.release();
-      st.taps_pq.release();
-      st.buf.release();
-    }
-    carry_raw.release();
-    staging.release();
-    d_out.release();
-    h_out.release();
-    if (stream) cudaStreamDestroy(stream);
-  }
   size_t raw_bytes() const { return iq_format == B2S_IQ_CS8 ? 2 : 8; }
 };
 
 // one Recorder: a bank of one channel that keeps no chunks
 struct b2s_recorder {
-  b2s_recorder_bank* bank = nullptr;
-  ~b2s_recorder() { delete bank; }
+  std::unique_ptr<b2s_recorder_bank> bank;
 };
 
 namespace {
@@ -511,10 +520,9 @@ void start_channel(b2s_recorder_bank::Channel& c, unsigned long long phase_inc) 
 }
 
 int bank_create(b2s_engine* e, int32_t sample_rate_hz, int32_t bandwidth_hz, int iq_format, float iq_scale, int flags, int n_channels, size_t max_samples_per_push,
-                bool keep_chunks, b2s_recorder_bank** out) {
-  *out = nullptr;
+                bool keep_chunks, std::unique_ptr<b2s_recorder_bank>& out) {
   CU(cudaSetDevice(e->device));
-  auto* k = new b2s_recorder_bank();
+  auto k = std::make_unique<b2s_recorder_bank>();
   k->engine = e;
   k->sample_rate = sample_rate_hz;
   k->bandwidth = bandwidth_hz;
@@ -526,12 +534,11 @@ int bank_create(b2s_engine* e, int32_t sample_rate_hz, int32_t bandwidth_hz, int
   k->n_ch = n_channels;
   k->chunk_samples = static_cast<int>((static_cast<long long>(bandwidth_hz) * 100 / 1000 + 4095) / 4096 * 4096);  // RECORDER_FLUSH_INTERVAL = 100 ms
   k->ch.resize(n_channels);
-  int rc = 0;
-  cudaError_t err = cudaStreamCreateWithFlags(&k->stream, cudaStreamNonBlocking);
-  if (err != cudaSuccess) rc = fail(B2S_E_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(err));
+  const cudaError_t err = cudaStreamCreateWithFlags(&k->stream.h, cudaStreamNonBlocking);
+  if (err != cudaSuccess) return fail(B2S_E_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(err));
+  int rc;
   size_t n_in = k->max_in;
   for (const auto& f : host::resamplers_factors(sample_rate_hz, bandwidth_hz, 125)) {  // RESAMPLER_THRESHOLD, config.h
-    if (rc) break;
     k->stages.emplace_back();
     auto& st = k->stages.back();
     st.interp = f.first;
@@ -541,28 +548,24 @@ int bank_create(b2s_engine* e, int32_t sample_rate_hz, int32_t bandwidth_hz, int
     st.hc = (st.n_taps - 1 + st.decim) / st.interp + 2;
     st.max_in = n_in;
     st.stride = st.hc + n_in + 2;
-    if (st.hc > 4096) rc = fail(B2S_E_INVALID, "resampler stage %d/%d needs %d samples of history", st.interp, st.decim, st.hc);
-    if (!rc) rc = st.taps.alloc(st.n_taps);
-    if (!rc && cudaMemcpy(st.taps.p, st.h_taps.data(), sizeof(float) * st.n_taps, cudaMemcpyHostToDevice) != cudaSuccess) rc = fail(B2S_E_CUDA, "taps upload failed");
-    if (!rc && st.interp == 1 && st.decim >= 2 && (st.n_taps + st.decim - 1) / st.decim <= kPolyQ) {
+    if (st.hc > 4096) return fail(B2S_E_INVALID, "resampler stage %d/%d needs %d samples of history", st.interp, st.decim, st.hc);
+    if ((rc = st.taps.alloc(st.n_taps))) return rc;
+    if (cudaMemcpy(st.taps.p, st.h_taps.data(), sizeof(float) * st.n_taps, cudaMemcpyHostToDevice) != cudaSuccess) return fail(B2S_E_CUDA, "taps upload failed");
+    if (st.interp == 1 && st.decim >= 2 && (st.n_taps + st.decim - 1) / st.decim <= kPolyQ) {
       std::vector<float> pq(static_cast<size_t>(st.decim) * kPolyQ, 0.0f);  // h[q D + p] at [p][q], zero padded
       for (int i = 0; i < st.n_taps; ++i) pq[static_cast<size_t>(i % st.decim) * kPolyQ + i / st.decim] = st.h_taps[i];
-      rc = st.taps_pq.alloc(pq.size());
-      if (!rc && cudaMemcpy(st.taps_pq.p, pq.data(), sizeof(float) * pq.size(), cudaMemcpyHostToDevice) != cudaSuccess) rc = fail(B2S_E_CUDA, "taps upload failed");
+      if ((rc = st.taps_pq.alloc(pq.size()))) return rc;
+      if (cudaMemcpy(st.taps_pq.p, pq.data(), sizeof(float) * pq.size(), cudaMemcpyHostToDevice) != cudaSuccess) return fail(B2S_E_CUDA, "taps upload failed");
     }
-    if (!rc && k->stages.size() > 1) rc = st.buf.alloc(st.stride * n_channels);
+    if (k->stages.size() > 1 && (rc = st.buf.alloc(st.stride * n_channels))) return rc;
     n_in = (n_in * st.interp) / st.decim + 2;
   }
   k->out_stride = n_in;
-  if (!rc) rc = k->carry_raw.alloc(static_cast<size_t>(k->stages[0].hc) * k->raw_bytes());
-  if (!rc) rc = k->d_out.alloc(2 * k->out_stride * n_channels);
-  if (!rc) rc = k->h_out.alloc(2 * k->out_stride * n_channels);
-  if (!rc && !k->on_device) rc = k->staging.alloc(k->max_in * k->raw_bytes());
-  if (rc) {
-    delete k;
-    return rc;
-  }
-  *out = k;
+  if ((rc = k->carry_raw.alloc(static_cast<size_t>(k->stages[0].hc) * k->raw_bytes()))) return rc;
+  if ((rc = k->d_out.alloc(2 * k->out_stride * n_channels))) return rc;
+  if ((rc = k->h_out.alloc(2 * k->out_stride * n_channels))) return rc;
+  if (!k->on_device && (rc = k->staging.alloc(k->max_in * k->raw_bytes()))) return rc;
+  out = std::move(k);
   return 0;
 }
 
@@ -688,13 +691,6 @@ struct b2s_averager {
   b2s_engine* engine = nullptr;
   int size = 0, group = 0, frames = 0, cur = 0;
   DevBuf<float> sum, ring[2], avg, rows;
-  ~b2s_averager() {
-    sum.release();
-    ring[0].release();
-    ring[1].release();
-    avg.release();
-    rows.release();
-  }
   int reset() {
     CU(cudaMemset(sum.p, 0, sizeof(float) * size));
     CU(cudaMemset(ring[0].p, 0, sizeof(float) * size * group));
@@ -730,17 +726,14 @@ int b2s_engine_create(int cuda_device, b2s_engine** out) {
   cudaError_t err = cudaGetDeviceCount(&count);
   if (err != cudaSuccess || count == 0) return fail(B2S_E_CUDA, "no usable CUDA device (%s); this engine has no CPU fallback", cudaGetErrorString(err));
   if (cuda_device < 0 || cuda_device >= count) return fail(B2S_E_INVALID, "cuda_device %d out of range (0..%d)", cuda_device, count - 1);
-  b2s_engine* e = new b2s_engine();
+  auto e = std::make_unique<b2s_engine>();
   e->device = cuda_device;
   CU(cudaSetDevice(cuda_device));
   CU(cudaGetDeviceProperties(&e->prop, cuda_device));
-  if (e->prop.major != 9 || e->prop.minor != 0) {  // sm_90a code runs on compute capability 9.0 and nothing else
-    const int major = e->prop.major, minor = e->prop.minor;
-    delete e;
-    return fail(B2S_E_CUDA, "device is sm_%d%d; this build targets sm_90a (H100) only", major, minor);
-  }
+  if (e->prop.major != 9 || e->prop.minor != 0)  // sm_90a code runs on compute capability 9.0 and nothing else
+    return fail(B2S_E_CUDA, "device is sm_%d%d; this build targets sm_90a (H100) only", e->prop.major, e->prop.minor);
   e->sm_count = e->prop.multiProcessorCount;
-  *out = e;
+  *out = e.release();
   return 0;
 }
 int b2s_engine_destroy(b2s_engine* e) {
@@ -787,13 +780,9 @@ int b2s_band_create(b2s_engine* e, const b2s_band_config* cfg, b2s_band** out) {
   *out = nullptr;
   int rc = validate_config(*cfg);
   if (rc) return rc;
-  b2s_band* b = new b2s_band();
-  rc = b->init(e, *cfg);
-  if (rc) {
-    delete b;
-    return rc;
-  }
-  *out = b;
+  auto b = std::make_unique<b2s_band>();
+  if ((rc = b->init(e, *cfg))) return rc;
+  *out = b.release();
   return 0;
 }
 int b2s_band_destroy(b2s_band* b) {
@@ -846,9 +835,9 @@ int b2s_band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, d
   const size_t pipe = b->async_mode ? std::min<size_t>(b->max_frames, std::max<size_t>(n_frames, 1))
                                     : std::max<size_t>(1, std::min<size_t>(b->max_frames, n_frames >= 512 ? (n_frames + 3) / 4 : n_frames));
   if (!b->copy_stream) {
-    CU(cudaStreamCreateWithFlags(&b->copy_stream, cudaStreamNonBlocking));
-    CU(cudaEventCreateWithFlags(&b->copy_done[0], cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&b->copy_done[1], cudaEventDisableTiming));
+    CU(cudaStreamCreateWithFlags(&b->copy_stream.h, cudaStreamNonBlocking));
+    CU(cudaEventCreateWithFlags(&b->copy_done[0].h, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&b->copy_done[1].h, cudaEventDisableTiming));
   }
   const size_t buf_bytes = pipe * stride_bytes;
   for (int i = 0; i < 2; ++i) {
@@ -1047,7 +1036,7 @@ int b2s_band_get_signals(b2s_band* b, int32_t* keys, int64_t* first, int64_t* la
 int b2s_averager_create(b2s_engine* e, int size, int group_size, b2s_averager** out) {
   if (!e || !out || size < 1 || group_size < 1) return fail(B2S_E_INVALID, "bad argument");
   CU(cudaSetDevice(e->device));
-  b2s_averager* a = new b2s_averager();
+  auto a = std::make_unique<b2s_averager>();
   a->engine = e;
   a->size = size;
   a->group = group_size;
@@ -1056,11 +1045,8 @@ int b2s_averager_create(b2s_engine* e, int size, int group_size, b2s_averager** 
   if (!rc) rc = a->ring[1].alloc(static_cast<size_t>(size) * group_size);
   if (!rc) rc = a->avg.alloc(size);
   if (!rc) rc = a->reset();
-  if (rc) {
-    delete a;
-    return rc;
-  }
-  *out = a;
+  if (rc) return rc;
+  *out = a.release();
   return 0;
 }
 int b2s_averager_destroy(b2s_averager* a) {
@@ -1110,25 +1096,16 @@ int b2s_average(b2s_engine* e, const float* in, float* out, int size, int group_
   DevBuf<float> din, dout;
   int rc = din.alloc(static_cast<size_t>(size) * rows);
   if (!rc) rc = dout.alloc(static_cast<size_t>(size) * rows);
-  if (rc) {
-    din.release();
-    dout.release();
-    return rc;
+  if (rc) return rc;
+  CU(cudaMemcpy(din.p, in, sizeof(float) * size * rows, cudaMemcpyHostToDevice));
+  if (exact) {
+    k_boxcar_serial<<<(rows + 31) / 32, 32>>>(din.p, dout.p, size, group_size, rows);
+  } else {
+    dim3 grid((size + 127) / 128, rows);
+    k_boxcar<<<grid, 128>>>(din.p, dout.p, size, group_size, rows);
   }
-  cudaError_t err = cudaMemcpy(din.p, in, sizeof(float) * size * rows, cudaMemcpyHostToDevice);
-  if (err == cudaSuccess) {
-    if (exact) {
-      k_boxcar_serial<<<(rows + 31) / 32, 32>>>(din.p, dout.p, size, group_size, rows);
-    } else {
-      dim3 grid((size + 127) / 128, rows);
-      k_boxcar<<<grid, 128>>>(din.p, dout.p, size, group_size, rows);
-    }
-    err = cudaGetLastError();
-  }
-  if (err == cudaSuccess) err = cudaMemcpy(out, dout.p, sizeof(float) * size * rows, cudaMemcpyDeviceToHost);
-  din.release();
-  dout.release();
-  if (err != cudaSuccess) return fail(B2S_E_CUDA, "b2s_average: %s", cudaGetErrorString(err));
+  CU(cudaGetLastError());
+  CU(cudaMemcpy(out, dout.p, sizeof(float) * size * rows, cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -1158,34 +1135,23 @@ int b2s_psd(b2s_engine* e, const b2s_band_config* cfg, const void* iq, size_t n_
   if (!rc) rc = dpv.alloc(n_frames);
   if (!rc) rc = dpi.alloc(n_frames);
   if (!rc && tables.split > 1) rc = dpacked.alloc(n_frames);
-  cudaError_t err = cudaSuccess;
-  if (!rc) err = cudaMemcpy(diq.p, iq, bytes, cudaMemcpyHostToDevice);
-  if (!rc && err == cudaSuccess) {
-    SpectralArgs sa{};
-    sa.iq = diq.p;
-    sa.frame_stride_bytes = static_cast<long long>(stride);
-    sa.n_frames = static_cast<int>(n_frames);
-    tables.fill(sa);
-    sa.inv_fs = 1.0f / static_cast<float>(c.sample_rate_hz);
-    sa.psd_db = dpsd.p;
-    sa.power_lin = power_lin ? dlin.p : nullptr;
-    sa.peak_index = dpi.p;
-    sa.peak_value = dpv.p;
-    sa.peak_packed = dpacked.p;
-    rc = launch_spectrum(e, c.fft_size, c.iq_format, sa, nullptr);
-    if (!rc) err = cudaDeviceSynchronize();
-    if (!rc && err == cudaSuccess) err = cudaMemcpy(psd_db, dpsd.p, sizeof(float) * n_frames * n, cudaMemcpyDeviceToHost);
-    if (!rc && err == cudaSuccess && power_lin) err = cudaMemcpy(power_lin, dlin.p, sizeof(float) * n_frames * n, cudaMemcpyDeviceToHost);
-  }
-  tables.release();
-  diq.release();
-  dpsd.release();
-  dlin.release();
-  dpv.release();
-  dpi.release();
-  dpacked.release();
   if (rc) return rc;
-  if (err != cudaSuccess) return fail(B2S_E_CUDA, "b2s_psd: %s", cudaGetErrorString(err));
+  CU(cudaMemcpy(diq.p, iq, bytes, cudaMemcpyHostToDevice));
+  SpectralArgs sa{};
+  sa.iq = diq.p;
+  sa.frame_stride_bytes = static_cast<long long>(stride);
+  sa.n_frames = static_cast<int>(n_frames);
+  tables.fill(sa);
+  sa.inv_fs = 1.0f / static_cast<float>(c.sample_rate_hz);
+  sa.psd_db = dpsd.p;
+  sa.power_lin = power_lin ? dlin.p : nullptr;
+  sa.peak_index = dpi.p;
+  sa.peak_value = dpv.p;
+  sa.peak_packed = dpacked.p;
+  if ((rc = launch_spectrum(e, c.fft_size, c.iq_format, sa, nullptr))) return rc;
+  CU(cudaDeviceSynchronize());
+  CU(cudaMemcpy(psd_db, dpsd.p, sizeof(float) * n_frames * n, cudaMemcpyDeviceToHost));
+  if (power_lin) CU(cudaMemcpy(power_lin, dlin.p, sizeof(float) * n_frames * n, cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -1251,11 +1217,10 @@ int b2s_recorder_create(b2s_engine* e, int32_t sample_rate_hz, int32_t bandwidth
   if (!e || !out || sample_rate_hz <= 0 || bandwidth_hz <= 0 || bandwidth_hz > sample_rate_hz) return fail(B2S_E_INVALID, "b2s_recorder_create: bad argument");
   if (iq_format != B2S_IQ_CS8 && iq_format != B2S_IQ_CF32) return fail(B2S_E_INVALID, "unknown iq_format %d", iq_format);
   *out = nullptr;
-  b2s_recorder_bank* k = nullptr;
-  const int rc = bank_create(e, sample_rate_hz, bandwidth_hz, iq_format, iq_scale, flags, 1, max_samples_per_push, false, &k);
+  auto r = std::make_unique<b2s_recorder>();
+  const int rc = bank_create(e, sample_rate_hz, bandwidth_hz, iq_format, iq_scale, flags, 1, max_samples_per_push, false, r->bank);
   if (rc) return rc;
-  *out = new b2s_recorder();
-  (*out)->bank = k;
+  *out = r.release();
   return 0;
 }
 int b2s_recorder_destroy(b2s_recorder* r) {
@@ -1296,7 +1261,7 @@ int b2s_recorder_push(b2s_recorder* r, const void* iq, size_t n_samples, int8_t*
   if (!r || (!iq && n_samples) || !n_out) return fail(B2S_E_INVALID, "b2s_recorder_push: NULL argument");
   *n_out = 0;
   if (!r->bank->ch[0].recording) return fail(B2S_E_STATE, "b2s_recorder_push: the recorder is not recording (b2s_recorder_start)");
-  return bank_push(r->bank, iq, n_samples, 0, out_iq, cap_samples, true, n_out, "b2s_recorder_push");
+  return bank_push(r->bank.get(), iq, n_samples, 0, out_iq, cap_samples, true, n_out, "b2s_recorder_push");
 }
 
 // ---- recorder bank: SdrDevice's recorders on one stream (sdr_device.cpp:39-41,82-144) ----
@@ -1305,7 +1270,12 @@ int b2s_recorder_bank_create(b2s_engine* e, int32_t sample_rate_hz, int32_t band
   if (!e || !out || sample_rate_hz <= 0 || bandwidth_hz <= 0 || bandwidth_hz > sample_rate_hz || n_channels <= 0)
     return fail(B2S_E_INVALID, "b2s_recorder_bank_create: bad argument");
   if (iq_format != B2S_IQ_CS8 && iq_format != B2S_IQ_CF32) return fail(B2S_E_INVALID, "unknown iq_format %d", iq_format);
-  return bank_create(e, sample_rate_hz, bandwidth_hz, iq_format, iq_scale, flags, n_channels, max_samples_per_push, true, out);
+  *out = nullptr;
+  std::unique_ptr<b2s_recorder_bank> k;
+  const int rc = bank_create(e, sample_rate_hz, bandwidth_hz, iq_format, iq_scale, flags, n_channels, max_samples_per_push, true, k);
+  if (rc) return rc;
+  *out = k.release();
+  return 0;
 }
 int b2s_recorder_bank_destroy(b2s_recorder_bank* k) {
   if (k) {
@@ -1363,7 +1333,7 @@ int b2s_selftest_div_const(b2s_engine* e, int divisor, uint64_t* mismatches) {
   DevBuf<unsigned long long> bad;
   int rc = bad.alloc(1);
   if (rc) return rc;
-  cudaMemset(bad.p, 0, sizeof(unsigned long long));
+  CU(cudaMemset(bad.p, 0, sizeof(unsigned long long)));
   switch (divisor) {
     case 2: rc = run_div_check<2>(e, bad.p); break;
     case 3: rc = run_div_check<3>(e, bad.p); break;
@@ -1378,12 +1348,9 @@ int b2s_selftest_div_const(b2s_engine* e, int divisor, uint64_t* mismatches) {
     case 21: rc = run_div_check<21>(e, bad.p); break;
     default: rc = fail(B2S_E_INVALID, "no div_const instantiation for divisor %d", divisor);
   }
-  unsigned long long h = 0;
-  cudaError_t err = cudaSuccess;
-  if (!rc) err = cudaMemcpy(&h, bad.p, sizeof(h), cudaMemcpyDeviceToHost);
-  bad.release();
   if (rc) return rc;
-  if (err != cudaSuccess) return fail(B2S_E_CUDA, "b2s_selftest_div_const: %s", cudaGetErrorString(err));
+  unsigned long long h = 0;
+  CU(cudaMemcpy(&h, bad.p, sizeof(h), cudaMemcpyDeviceToHost));
   *mismatches = h;
   return 0;
 }
@@ -1464,7 +1431,7 @@ int b2s_host_transmission_create(const b2s_band_config* cfg, b2s_host_transmissi
   if (!cfg || !out) return fail(B2S_E_INVALID, "NULL argument");
   int rc = validate_config(*cfg);
   if (rc) return rc;
-  auto* h = new b2s_host_transmission();
+  auto h = std::make_unique<b2s_host_transmission>();
   h->cfg = *cfg;
   h->cfg.window_taps = nullptr;
   TrackerParams& p = h->tracker.p;
@@ -1487,7 +1454,7 @@ int b2s_host_transmission_create(const b2s_band_config* cfg, b2s_host_transmissi
   p.timeout = cfg->timeout_ms;
   p.max_time = cfg->max_time_ms;
   h->history.assign(static_cast<size_t>(cfg->grouping_y) * cfg->fft_size, 0.0f);  // Averager::reset fills the ring with zeros
-  *out = h;
+  *out = h.release();
   return 0;
 }
 int b2s_host_transmission_destroy(b2s_host_transmission* h) {

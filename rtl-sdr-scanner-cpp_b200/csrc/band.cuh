@@ -1,5 +1,5 @@
 // b2s_band: per-band state, the two halves of a push (GPU enqueue / result finish) and the optional result worker.
-// Included by b2s_api.cu after its helpers (fail, CU, DevBuf, PinBuf, launch_spectrum, SpectralTables).
+// Included by b2s_api.cu after its helpers (fail, CU, DevBuf, PinBuf, Stream, Event, launch_spectrum, SpectralTables).
 //
 // A push (or each pipeline chunk of one) goes through
 //   enqueue_chunk : K1 -> K2 -> entry ordering on the band's stream, non-blocking on the host
@@ -55,7 +55,7 @@ struct PushSlot {
   DevBuf<int> run_lo, run_hi, run_count;  // RunFold arrays of the chunk
   DevBuf<TrackResult> d_result;
   PinBuf<TrackResult> h_result;
-  cudaEvent_t sorted_done = nullptr, tev[2] = {nullptr, nullptr};
+  Event sorted_done, tev[2];
   bool host_track = false;  // this chunk's bookkeeping runs on the host (the caller asked for every frame's list)
   int epoch = 0;            // reset_epoch when the chunk was enqueued
   PinBuf<int> h_offsets, h_cand_flag;
@@ -63,7 +63,7 @@ struct PushSlot {
   PinBuf<DetectEntry> h_entries;
   int n_watch = 0;
   int watch_key[kMaxWatch] = {0};
-  cudaEvent_t gpu_done = nullptr, ev[4] = {nullptr, nullptr, nullptr, nullptr};
+  Event gpu_done, ev[4];
   // context of the chunk in flight
   bool busy = false;
   int T = 0;
@@ -79,30 +79,18 @@ struct PushSlot {
   b2s_result* out = nullptr;  // synchronous mode only
   std::vector<float> thr_host;
   bool thr_host_valid = false;
-  void release() {
-    psd.release(); ckpt.release(); dense_q.release(); dense_avg.release(); dense_box.release(); peak_val.release();
-    peak_idx.release(); offsets.release(); max_count.release(); sorted.release(); spec_rows.release();
-    box_last.release(); run_lo.release(); run_hi.release(); run_count.release(); d_result.release(); h_result.release();
-    if (sorted_done) cudaEventDestroy(sorted_done);
-    for (auto& e : tev) {
-      if (e) cudaEventDestroy(e);
-    }
-    h_offsets.release(); h_entries.release(); watch_max.release(); cta_ns.release(); peak_packed.release(); cand_flag.release(); h_cand_flag.release(); h_watch_max.release();
-    if (gpu_done) cudaEventDestroy(gpu_done);
-    for (auto& e : ev) {
-      if (e) cudaEventDestroy(e);
-    }
-  }
 };
 
 struct b2s_band : public DeviceQueries {
   b2s_engine* engine = nullptr;
   b2s_band_config cfg{};
   std::mutex mutex;  // serialises API calls on this band
-  cudaStream_t own_stream = nullptr, stream = nullptr, finish_stream = nullptr, copy_stream = nullptr;
-  cudaStream_t track_stream = nullptr;  // K4 of push k runs here, beside K1 of push k+1 on `stream`
-  DevBuf<TrackState> d_state;           // the signal map (device resident; tracker.signals mirrors it only inside a host-tracked push)
-  cudaEvent_t copy_done[2] = {nullptr, nullptr}, iq_prev_use[2] = {nullptr, nullptr};
+  // The streams are declared before every buffer, so they are destroyed after them.
+  Stream own_stream, finish_stream, copy_stream;
+  Stream track_stream;            // K4 of push k runs here, beside K1 of push k+1 on `stream`
+  cudaStream_t stream = nullptr;  // own_stream, or the caller's stream (b2s_band_set_stream)
+  DevBuf<TrackState> d_state;     // the signal map (device resident; tracker.signals mirrors it only inside a host-tracked push)
+  Event copy_done[2], iq_prev_use[2];
   int iq_slot = 0;
   int max_frames = 0;
   int slot_capacity = 0;  // detection entries per frame
@@ -152,30 +140,9 @@ struct b2s_band : public DeviceQueries {
   PushSlot* cur = nullptr;  // slot whose finish half is running (DeviceQueries context)
   cudaStream_t fstream() const { return async_mode ? finish_stream : stream; }
 
-  ~b2s_band() {
-    shutdown_worker();
-    tables.release();
-    d_iq[0].release(); d_iq[1].release(); d_sum[0].release(); d_sum[1].release(); d_avg_last.release();
-    for (auto& r : d_ring) r.release();
-    d_slots.release(); d_slot_count.release(); d_wq_val.release(); d_wq_idx.release(); h_work.release();
-    for (auto& s : slots) s.release();
-    for (auto& kv : noise) {
-      kv.second.threshold[0].release();
-      kv.second.threshold[1].release();
-    }
-    for (auto& kv : spectro) kv.second.sum.release();
-    for (auto& e : copy_done) {
-      if (e) cudaEventDestroy(e);
-    }
-    for (auto& e : iq_prev_use) {
-      if (e) cudaEventDestroy(e);
-    }
-    d_state.release();
-    if (track_stream) cudaStreamDestroy(track_stream);
-    if (copy_stream) cudaStreamDestroy(copy_stream);
-    if (finish_stream) cudaStreamDestroy(finish_stream);
-    if (own_stream) cudaStreamDestroy(own_stream);
-  }
+  // The worker reads the slots and the band's state until it stops: join it before any member is destroyed. The members then
+  // free themselves.
+  ~b2s_band() { shutdown_worker(); }
 
   // ---------------------------------------------------------------------------------------------------------
   int noise_slot(NoiseSlot** out) {
@@ -276,10 +243,10 @@ struct b2s_band : public DeviceQueries {
       if (rc2) return rc2;
       if (smem > 64 * 1024) return fail(B2S_E_INVALID, "window query of %zu bytes exceeds the kernel's shared-memory budget", smem);
     }
-    cudaEvent_t w0 = nullptr, w1 = nullptr;
+    Event w0, w1;
     if (profiling) {
-      CU(cudaEventCreate(&w0));
-      CU(cudaEventCreate(&w1));
+      CU(cudaEventCreate(&w0.h));
+      CU(cudaEventCreate(&w1.h));
       CU(cudaEventRecord(w0, st));
     }
     k_window_query<<<static_cast<unsigned>(work.size()), 256, smem, st>>>(a);
@@ -296,8 +263,6 @@ struct b2s_band : public DeviceQueries {
       float ms = 0.0f;
       CU(cudaEventElapsedTime(&ms, w0, w1));
       prof.window_ms += ms;
-      cudaEventDestroy(w0);
-      cudaEventDestroy(w1);
     }
     values.resize(w.size());
     indices.resize(w.size());
@@ -321,9 +286,9 @@ struct b2s_band : public DeviceQueries {
     slot_capacity = c.detect_capacity > 0 ? c.detect_capacity : std::max(256, std::min(4096, c.fft_size / 8));
     async_mode = (c.flags & B2S_FLAG_ASYNC) != 0;
     center = c.center_hz;
-    CU(cudaStreamCreateWithFlags(&own_stream, cudaStreamNonBlocking));
-    CU(cudaStreamCreateWithFlags(&finish_stream, cudaStreamNonBlocking));
-    CU(cudaStreamCreateWithFlags(&track_stream, cudaStreamNonBlocking));
+    CU(cudaStreamCreateWithFlags(&own_stream.h, cudaStreamNonBlocking));
+    CU(cudaStreamCreateWithFlags(&finish_stream.h, cudaStreamNonBlocking));
+    CU(cudaStreamCreateWithFlags(&track_stream.h, cudaStreamNonBlocking));
     stream = own_stream;
     int rc = tables.build(c);
     if (rc) return rc;
@@ -381,8 +346,8 @@ struct b2s_band : public DeviceQueries {
       if ((rc = s.cand_flag.alloc(max_frames))) return rc;
       if ((rc = s.h_watch_max.alloc(static_cast<size_t>(max_frames) * kMaxWatch))) return rc;
       if ((rc = s.h_cand_flag.alloc(max_frames))) return rc;
-      CU(cudaEventCreateWithFlags(&s.gpu_done, cudaEventDisableTiming));
-      CU(cudaEventCreateWithFlags(&s.sorted_done, cudaEventDisableTiming));
+      CU(cudaEventCreateWithFlags(&s.gpu_done.h, cudaEventDisableTiming));
+      CU(cudaEventCreateWithFlags(&s.sorted_done.h, cudaEventDisableTiming));
       if ((rc = s.box_last.alloc(n))) return rc;
       if ((rc = s.run_lo.alloc(static_cast<size_t>(2 * kRunCap) * max_frames))) return rc;
       if ((rc = s.run_hi.alloc(static_cast<size_t>(2 * kRunCap) * max_frames))) return rc;
@@ -423,7 +388,7 @@ struct b2s_band : public DeviceQueries {
     p.max_time = c.max_time_ms;
     if (async_mode) {
       for (int i = 0; i < 2; ++i) {
-        CU(cudaEventCreateWithFlags(&iq_prev_use[i], cudaEventDisableTiming));
+        CU(cudaEventCreateWithFlags(&iq_prev_use[i].h, cudaEventDisableTiming));
         CU(cudaEventRecord(iq_prev_use[i], stream));
       }
       worker = std::thread([this]() { worker_loop(); });
@@ -661,7 +626,7 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
   if (s.dense_box_on && (rc = s.dense_box.alloc(static_cast<size_t>(max_frames) * n))) return rc;
   if (profiling) {
     for (auto& e : s.ev) {
-      if (!e) CU(cudaEventCreate(&e));
+      if (!e) CU(cudaEventCreate(&e.h));
     }
   }
 
@@ -881,7 +846,7 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
     if ((rc = prepare_kernel(engine, k_track, kTrackThreads, sizeof(TrackShared), nullptr))) return rc;
     if (profiling) {
       for (auto& e : s.tev) {
-        if (!e) CU(cudaEventCreate(&e));
+        if (!e) CU(cudaEventCreate(&e.h));
       }
       CU(cudaEventRecord(s.tev[0], track_stream));
     }
