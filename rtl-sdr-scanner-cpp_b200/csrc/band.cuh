@@ -738,8 +738,9 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
   da.avg_last = d_avg_last.p;
   da.checkpoints = s.ckpt.p;
   da.detect_level = std::min(cfg.start_level, cfg.stop_level);
-  da.detect_sum = least_sum_reaching(da.detect_level, cfg.grouping_x);
-  da.start_sum = least_sum_reaching(cfg.start_level, cfg.grouping_x);
+  // an interior boxcar window holds 2 * (X / 2) + 1 bins (X + 1 for an even X), and that is what its sum is divided by
+  da.detect_sum = least_sum_reaching(da.detect_level, 2 * (cfg.grouping_x / 2) + 1);
+  da.start_sum = least_sum_reaching(cfg.start_level, 2 * (cfg.grouping_x / 2) + 1);
   da.slots = d_slots.p;
   da.slot_count = d_slot_count.p;
   da.slot_capacity = slot_capacity;

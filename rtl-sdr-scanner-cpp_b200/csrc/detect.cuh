@@ -68,7 +68,8 @@ struct DetectArgs {
   float* checkpoints;     // [ceil(T/64)][N] m_sum before frame 64*c
   // detection: per-frame slot lists
   float detect_level;     // min(start, stop)
-  // the same two levels as thresholds on the UNDIVIDED boxcar sum of an interior bin: x >= detect_sum  <=>  x / X >= detect_level
+  // the same two levels as thresholds on the UNDIVIDED boxcar sum of an interior bin, whose window holds XD = 2 * (X / 2) + 1 bins
+  // (X + 1 for an even X): x >= detect_sum  <=>  x / XD >= detect_level
   // (IEEE division is monotonic, so the set {x : fl(x / X) >= level} is an upper interval; the host finds its least element)
   float detect_sum, start_sum;
   DetectEntry* slots;     // [ceil(T/32)][slot_capacity][32], see slot_index()
