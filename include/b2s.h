@@ -62,8 +62,8 @@ extern "C" {
 /* Construction-time parameters. The reference takes them from Config / Device / the setupChains lambdas
  * (sdr_device.cpp:148-167, transmission.h:17-25, config.h:24-38). */
 typedef struct b2s_band_config {
-  int32_t fft_size;             /* N = getFft(fs, SIGNAL_DETECTION_MAX_STEP); power of two, 256..262144 (sizes above 16384 run as 16384-point
-                                   residue classes of the bin index, see csrc/spectral3.cuh) */
+  int32_t fft_size;             /* N = getFft(fs, SIGNAL_DETECTION_MAX_STEP); power of two, 256..1048576 (sizes above 16384 run as S = N/16384
+                                   16384-point residue classes of the bin index, S up to 64, see csrc/spectral3.cuh) */
   int32_t sample_rate_hz;       /* Device::m_sampleRate (Frequency = int32_t) */
   int32_t frame_stride_samples; /* fftSize * decimatorFactor complex samples between frame starts (sdr_device.cpp:161-163) */
   int32_t iq_format;            /* B2S_IQ_* */
@@ -90,7 +90,8 @@ typedef struct b2s_band_config {
   int64_t spectrogram_interval_ms; /* SPECTROGRAM_SEND_INTERVAL (1000) */
   int32_t flags;                /* B2S_FLAG_* */
   /* ---- engine-only sizing (ignored by the oracle) ---- */
-  int32_t max_frames_per_push;  /* capacity of the per-push device buffers; 0 -> 4096 */
+  int32_t max_frames_per_push;  /* capacity of the per-push device buffers; 0 -> 4096 for N <= 262144, 2^30 / N above (2048 at 524288,
+                                   1024 at 1048576). Above N = 262144, max_frames_per_push * N must not exceed 2^30 (4 GiB of PSD rows). */
   int32_t detect_capacity;      /* detection entries kept per FRAME (bins >= min(start,stop)); 0 -> clamp(N/8, 256, 4096); grows on overflow */
   /* ---- noise learning on the frame clock (read by the engine AND the oracle) ---- */
   int64_t noise_learning_ms;    /* > 0: NoiseLearner's own rule (noise_learner.cpp:11,23): a centre frequency is learned from its first frame

@@ -208,9 +208,14 @@ int launch_spectrum3_v(b2s_engine* e, const SpectralArgs& a, cudaStream_t stream
 }
 
 // Which K1 serves which FFT size: k_spectrum (Stockham, two barriers per pass) below 4096, k_spectrum3 (warp-local passes) for
-// 4096 / 8192 / 16384, and k_spectrum3's split mode (S residue classes x 16384 points) for 32768 ... 262144.
-constexpr int kMaxFft = 16 * kSplitM;
+// 4096 / 8192 / 16384, and k_spectrum3's split mode (S residue classes x 16384 points) for 32768 ... 1048576.
+constexpr int kMaxFft = 64 * kSplitM;
 constexpr bool k1_is_v3(int n) { return n >= 4096; }
+
+// A band's per-push PSD slot holds max_frames_per_push rows of N floats. The default is 4096 rows up to N = 262144; above
+// that, the default and the cap are 2^30 / N rows, so that no slot is larger than the 4 GiB of a default slot at 262144.
+constexpr long long kMaxPushBins = 1LL << 30;
+constexpr int default_max_frames(int n) { return n > 16 * kSplitM ? static_cast<int>(kMaxPushBins / n) : 4096; }
 
 template <int N, int MODE>
 int launch_spectrum_t(b2s_engine* e, const SpectralArgs& a, cudaStream_t stream) {
@@ -242,6 +247,8 @@ int launch_spectrum_n(b2s_engine* e, int n, const SpectralArgs& a, cudaStream_t 
     case 65536: return launch_spectrum_t<65536, MODE>(e, a, stream);
     case 131072: return launch_spectrum_t<131072, MODE>(e, a, stream);
     case 262144: return launch_spectrum_t<262144, MODE>(e, a, stream);
+    case 524288: return launch_spectrum_t<524288, MODE>(e, a, stream);
+    case 1048576: return launch_spectrum_t<1048576, MODE>(e, a, stream);
     default: return fail(B2S_E_INVALID, "fft_size %d is not supported (256..%d)", n, kMaxFft);
   }
 }
@@ -345,6 +352,9 @@ struct SpectralTables {
 
 int validate_config(const b2s_band_config& c) {
   if (!is_pow2(c.fft_size) || c.fft_size < 256 || c.fft_size > kMaxFft) return fail(B2S_E_INVALID, "fft_size must be a power of two in 256..%d (got %d)", kMaxFft, c.fft_size);
+  if (c.fft_size > 16 * kSplitM && static_cast<long long>(c.max_frames_per_push) * c.fft_size > kMaxPushBins)
+    return fail(B2S_E_INVALID, "max_frames_per_push %d at fft_size %d exceeds %d: one push's PSD rows would take more than 4 GiB of device memory",
+                c.max_frames_per_push, c.fft_size, default_max_frames(c.fft_size));
   if (c.sample_rate_hz <= 0) return fail(B2S_E_INVALID, "sample_rate_hz must be positive");
   if (c.frame_stride_samples < c.fft_size) return fail(B2S_E_INVALID, "frame_stride_samples (%d) < fft_size", c.frame_stride_samples);
   if (c.iq_format != B2S_IQ_CS8 && c.iq_format != B2S_IQ_CF32) return fail(B2S_E_INVALID, "unknown iq_format %d", c.iq_format);

@@ -279,7 +279,7 @@ struct b2s_band : public DeviceQueries {
     engine = e;
     cfg = c;
     CU(cudaSetDevice(e->device));
-    max_frames = c.max_frames_per_push > 0 ? c.max_frames_per_push : 4096;
+    max_frames = c.max_frames_per_push > 0 ? c.max_frames_per_push : default_max_frames(c.fft_size);
     // detection entries kept per frame: every bin of a wideband emitter is one (a 200 kHz FM carrier at 250 Hz/bin is 800), so the
     // default scales with N; an overflowing push still completes on the truncated lists, reports B2S_E_OVERFLOW and the
     // capacity grows before the next push (grow_capacity)
@@ -844,14 +844,15 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
     ta.ring_before = d_ring[ring_in].p;
     ta.state = d_state.p;
     ta.result = s.d_result.p;
-    if ((rc = prepare_kernel(engine, k_track, kTrackThreads, sizeof(TrackShared), nullptr))) return rc;
+    auto* track = run_len_bits(cfg.fft_size) == 14 ? k_track<14> : k_track<12>;
+    if ((rc = prepare_kernel(engine, track, kTrackThreads, sizeof(TrackShared), nullptr))) return rc;
     if (profiling) {
       for (auto& e : s.tev) {
         if (!e) CU(cudaEventCreate(&e.h));
       }
       CU(cudaEventRecord(s.tev[0], track_stream));
     }
-    k_track<<<1, kTrackThreads, sizeof(TrackShared), track_stream>>>(ta);
+    track<<<1, kTrackThreads, sizeof(TrackShared), track_stream>>>(ta);
     CU(cudaGetLastError());
     if (profiling) CU(cudaEventRecord(s.tev[1], track_stream));
     // the result header and the first B2S_MAX_TX transmissions (the rest, if any, is fetched by the finish half)

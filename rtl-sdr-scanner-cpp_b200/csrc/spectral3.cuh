@@ -114,18 +114,20 @@ constexpr int kSplitStageBytes = 32768; // one staging buffer: S row segments of
 // blockIdx-strided walk, so a CTA that starts late (another band's kernel still holds its SM, config 3 / 5) simply takes
 // fewer items; the kernel leaves the counter pair zeroed for the next launch.
 //
-// SPLIT (N = S * 16384, S = 2, 4, 8, 16 -> N = 32768 ... 262144): decimation in frequency over the S residue classes of
+// SPLIT (N = S * 16384, S = 2 ... 64 -> N = 32768 ... 1048576): decimation in frequency over the S residue classes of
 // the bin index. Item (frame, c) computes
 //        y_c[n'] = W_N^(n' c) * sum_s x[n' + 16384 s] w[n' + 16384 s] W_S^(s c),     n' < 16384        (pre-pass)
 // and X[S k' + c] = FFT_16384(y_c)[k'] with exactly the passes of the non-split kernel. The S items of one frame are
 // adjacent in the work order: they read the same int8 frame (L2 hits after the first) and fill the same output sectors.
-// The int8 frame reaches the pre-pass through a 2-stage ring of bulk copies (S row segments per stage).
+// The int8 frame reaches the pre-pass through a 2-stage ring of bulk copies (S row segments of 16384 / S samples per
+// stage, so a stage stays kSplitStageBytes whatever S is); at S = 64 a stage has fewer points than the CTA has threads,
+// and two threads share each point.
 template <int RA, int MODE, bool DEBUG_LIN, int SPLIT_S>
 __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
   constexpr bool SPLIT = SPLIT_S > 1;
   constexpr int M = RA * 1024, T = RA * 32, BPT = 32 / RA;  // sub-transform length, threads, pass-A butterflies per thread
   static_assert(!SPLIT || RA == 16, "the split mode runs 16384-point sub-transforms");
-  static_assert(SPLIT_S == 1 || SPLIT_S == 2 || SPLIT_S == 4 || SPLIT_S == 8 || SPLIT_S == 16, "S");
+  static_assert(SPLIT_S == 1 || SPLIT_S == 2 || SPLIT_S == 4 || SPLIT_S == 8 || SPLIT_S == 16 || SPLIT_S == 32 || SPLIT_S == 64, "S");
   extern __shared__ __align__(128) unsigned char smem[];
   using C = cpk;
   C* X = reinterpret_cast<C*>(smem);                                           // [RA][kBlockPitch]
@@ -136,7 +138,7 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
   __shared__ float red_v[32];
   __shared__ int red_i[2];
   __shared__ int s_item[2];
-  __shared__ float2 s_ws[16];
+  __shared__ float2 s_ws[SPLIT_S > 16 ? SPLIT_S : 16];
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const char* base = static_cast<const char*>(a.iq);
@@ -197,6 +199,22 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
       for (int q = 0; q < S; ++q) {
         const unsigned char* st = raw + (chunk_no & 1u) * kSplitStageBytes;
         if (MODE == kModeCs8Tma) mbar_wait(&full_bar[chunk_no & 1u], (chunk_no >> 1) & 1u);
+        // windowed sample n = np + 16384 s of the frame; i = np - q * pc is its column in the stage
+        auto term = [&](int i, int np, int s) {
+          const int n = np + s * M;
+          const float w = __ldg(&a.wscale[n]);
+          if (MODE == kModeCs8Tma) {
+            const char2 smp = reinterpret_cast<const char2*>(st + s * pc * 2)[i];
+            return cscale(cmake(C{}, static_cast<float>(smp.x), static_cast<float>(smp.y)), w);
+          } else if (MODE == kModeCs8Direct) {
+            const signed char* fp = reinterpret_cast<const signed char*>(base + static_cast<long long>(frame) * a.frame_stride_bytes);
+            return cscale(cmake(C{}, static_cast<float>(fp[2 * n]), static_cast<float>(fp[2 * n + 1])), w);
+          } else {
+            const float* fp = reinterpret_cast<const float*>(base + static_cast<long long>(frame) * a.frame_stride_bytes);
+            return cscale(cmake(C{}, fp[2 * n], fp[2 * n + 1]), w);
+          }
+        };
+        if constexpr (S <= 16) {
 #pragma unroll(S >= 8 ? 2 : 4)
         for (int u = 0; u < pc / T; ++u) {  // independent points: their loads overlap
           const int i = tid + u * T;
@@ -204,19 +222,7 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
           C acc = cmake(C{}, 0.0f, 0.0f);
 #pragma unroll
           for (int s = 0; s < S; ++s) {
-            const int n = np + s * M;
-            const float w = __ldg(&a.wscale[n]);
-            C xs;
-            if (MODE == kModeCs8Tma) {
-              const char2 smp = reinterpret_cast<const char2*>(st + s * pc * 2)[i];
-              xs = cscale(cmake(C{}, static_cast<float>(smp.x), static_cast<float>(smp.y)), w);
-            } else if (MODE == kModeCs8Direct) {
-              const signed char* fp = reinterpret_cast<const signed char*>(base + static_cast<long long>(frame) * a.frame_stride_bytes);
-              xs = cscale(cmake(C{}, static_cast<float>(fp[2 * n]), static_cast<float>(fp[2 * n + 1])), w);
-            } else {
-              const float* fp = reinterpret_cast<const float*>(base + static_cast<long long>(frame) * a.frame_stride_bytes);
-              xs = cscale(cmake(C{}, fp[2 * n], fp[2 * n + 1]), w);
-            }
+            const C xs = term(i, np, s);
             if (s == 0) {  // W_S^0 = 1
               acc = xs;
             } else if (S == 2) {  // W_2^c = +-1
@@ -227,6 +233,21 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
           }
           if (c != 0) acc = cmul(acc, __ldg(&twc[np]));
           X[(np >> 10) * kBlockPitch + (np & 1023)] = acc;
+        }
+        } else {
+          // S = 32, 64: a stage has pc = 512 or 256 points for T = 512 threads, and every thread sums 32 terms. At S = 32 a thread
+          // has one point. At S = 64 lanes l and l + 16 of a warp share a point: lane half h sums the terms s = 32 h ... 32 h + 31,
+          // and one shuffle adds the two halves.
+          constexpr int kLanes = T / pc, kPoints = 32 / kLanes, kTerms = S / kLanes;  // lanes per point, points per warp
+          static_assert(kLanes * pc == T && kTerms == 32, "one or two threads per point");
+          const int h = lane / kPoints, i = warp * kPoints + lane % kPoints;
+          const int np = q * pc + i, s0 = h * kTerms;
+          C acc = cmul(term(i, np, s0), s_ws[s0]);
+#pragma unroll
+          for (int s = 1; s < kTerms; ++s) acc = cmadd(term(i, np, s0 + s), s_ws[s0 + s], acc);
+          if (kLanes == 2) acc = cadd(acc, cmake(C{}, __shfl_xor_sync(0xffffffffu, cre(acc), 16), __shfl_xor_sync(0xffffffffu, cim(acc), 16)));
+          if (c != 0) acc = cmul(acc, __ldg(&twc[np]));
+          if (h == 0) X[(np >> 10) * kBlockPitch + (np & 1023)] = acc;
         }
         __syncthreads();  // this stage is consumed (and, after the last chunk, y_c is complete)
         if (MODE == kModeCs8Tma && tid == 0) {  // refill it with the chunk two ahead (possibly of the next item)

@@ -26,7 +26,9 @@
 namespace b2s {
 
 constexpr int kMaxSignals = 256;   // live signals per band held by K4; beyond it the push fails loudly (B2S_E_OVERFLOW)
-constexpr int kRunLenBits = 14;    // a run is packed as (first bin << 14) | (length - 1); longer stretches are cut into several runs
+// k_track packs a run into 32 bits as (first bin << LEN_BITS) | (length - 1), and replays a frame with a longer run from its raw
+// entries. The first bin takes the other 32 - LEN_BITS bits: LEN_BITS = 14 up to N = 2^18, 12 up to N = 2^20.
+constexpr int run_len_bits(int n) { return n > (1 << 18) ? 12 : 14; }
 constexpr int kTrackThreads = 1024, kTrackFrames = 1024, kTrackWords = kTrackFrames / 32;
 constexpr int kMaxCand = 2048;     // start-level candidates replayed in one event frame
 
@@ -202,7 +204,10 @@ __device__ void track_best_index(const TrackArgs& a, TrackShared& s, int index, 
   __syncthreads();
 }
 
+template <int LEN_BITS>
 __global__ void __launch_bounds__(kTrackThreads, 1) k_track(const TrackArgs a) {
+  static_assert(LEN_BITS == 12 || LEN_BITS == 14, "run_len_bits");
+  constexpr int kRunLenBits = LEN_BITS;
   extern __shared__ __align__(16) unsigned char track_smem[];
   TrackShared& s = *reinterpret_cast<TrackShared*>(track_smem);
   const TrackParams& p = a.p;

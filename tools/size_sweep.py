@@ -14,7 +14,7 @@ def main():
     import torch
 
     b2s, synth = ge.load_b2s(), ge.load_synth()
-    sizes = [int(x) for x in sys.argv[1:]] or [4096, 8192, 16384, 32768, 65536, 131072, 262144]
+    sizes = [int(x) for x in sys.argv[1:]] or [4096, 8192, 16384, 32768, 65536, 131072, 262144, 524288, 1048576]
     eng = b2s.Engine(0)
     dev = torch.device("cuda", 0)
     out = []
@@ -41,6 +41,7 @@ def main():
         p = band.get_profile(reset=True)
         k1, k2 = p.spectral_ms / p.spectral_launches, p.detect_ms / p.detect_launches
         row = {"n": n, "frames": T, "k1_ms": round(k1, 4), "k2_ms": round(k2, 4), "k1_gbs": round(6 * T * n / k1 / 1e6, 1), "k2_gbs": round(4 * T * n / k2 / 1e6, 1),
+               "k1_gsps": round(T * n / k1 / 1e6, 3), "k1k2_gsps": round(T * n / (k1 + k2) / 1e6, 3),
                "host_ms": round(p.tracker_host_ms / reps, 4), "k4_ms": round(p.track_ms / max(p.track_launches, 1), 4),
                "k4_evals": p.track_evals / max(p.track_launches, 1), "k4_events": p.track_events / max(p.track_launches, 1)}
         print(json.dumps(row), flush=True)
