@@ -319,6 +319,33 @@ int b2s_recorder_bank_push(b2s_recorder_bank* k, const void* iq, size_t n_sample
 int b2s_recorder_bank_flush(b2s_recorder_bank* k, int channel, int8_t* chunks /*[cap][chunk_samples][2]*/, int64_t* times_ms,
                             int cap, int consume, int* count, int* chunk_samples);
 
+/* Record from the band's own pushes: every later b2s_band_push also runs `bank` over the pushed stream, reading the IQ the band
+ * has already staged on the device (or the caller's device pointer). bank == NULL detaches. (SdrDevice connects its recorders to
+ * the same source as the detection chain, sdr_device.cpp:39-41.)
+ *   - Compatibility: the bank is on the band's engine, has the band's sample_rate_hz, iq_format and iq_scale, and its
+ *     max_samples_per_push is at least max_frames_per_push * frame_stride_samples. A band has at most one bank and a bank is attached
+ *     to at most one band; attaching a second bank is refused (detach first). Any other case returns B2S_E_INVALID and changes
+ *     neither object. The bank's own B2S_FLAG_IQ_ON_DEVICE does not matter while it is attached.
+ *   - What the bank sees: while a bank is attached, `iq` of b2s_band_push must hold the whole stream, n_frames * frame_stride_samples
+ *     samples (without a bank, (n_frames - 1) * frame_stride_samples + fft_size are enough). A push of up to max_frames_per_push
+ *     frames is exactly one bank push of n_frames * frame_stride_samples samples at the push's t0_ms; a longer push is cut every
+ *     max_frames_per_push frames, piece j stamped t0_ms + floor(j * max_frames_per_push * frame_period_ms + 0.5). The band's own
+ *     pipeline chunks and its cuts at the spectrogram emission limit do not show in the bank's pushes.
+ *   - One upload: host IQ crosses PCIe once (b2s_profile.h2d_bytes grows by n_frames * frame_stride_samples * bytes per sample per
+ *     push); the bank reads the band's copy. The band's results are those of the same band without a bank, bit for bit.
+ *   - Device input: as without a bank, `iq` may be reused in the band's stream order once the call returns: work enqueued on the
+ *     band's stream afterwards waits for the bank's reads of it, even when they are still running on the bank's own stream.
+ *   - Completion: with a synchronous band the bank has consumed the push when b2s_band_push returns. With B2S_FLAG_ASYNC, b2s_band_push
+ *     does not wait for the bank's kernels of the push's last piece; the bank's host side of that piece (the copy of the channels'
+ *     output, the chunks) is done by the next b2s_band_push, b2s_band_sync or b2s_recorder_bank_* call on the bank, whichever comes
+ *     first. start / stop act on the pushes after them, as for a stand-alone bank.
+ *   - An attached bank is externally synchronised with its band: its calls must not run concurrently with that band's push.
+ *   - Lifetimes: destroying an attached bank detaches it first (which drains the band's outstanding pushes); destroying a band
+ *     detaches its bank, which stays usable. After a detach the bank's stream position continues: a stand-alone b2s_recorder_bank_push
+ *     of the following samples continues the same recordings byte for byte. b2s_band_reset, b2s_band_set_center and noise learning do
+ *     not touch the bank. */
+int b2s_band_attach_recorder_bank(b2s_band* b, b2s_recorder_bank* bank);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import weakref
 from typing import Optional
 
 import numpy as np
@@ -191,6 +192,8 @@ def lib():
         L.b2s_band_create.argtypes = [C.c_void_p, C.POINTER(BandConfig), C.POINTER(C.c_void_p)]
         L.b2s_band_destroy.argtypes = [C.c_void_p]
         L.b2s_band_set_stream.argtypes = [C.c_void_p, C.c_void_p]
+        L.b2s_band_attach_recorder_bank.argtypes = [C.c_void_p, C.c_void_p]
+        L.b2s_band_attach_recorder_bank.restype = C.c_int
         L.b2s_band_reset.argtypes = [C.c_void_p]
         L.b2s_band_sync.argtypes = [C.c_void_p, C.POINTER(Result)]
         L.b2s_band_set_profiling.argtypes = [C.c_void_p, C.c_int]
@@ -352,7 +355,25 @@ class Band(_Handle):
         super().__init__(lib().b2s_band_destroy)
         self._e = engine
         self.cfg = cfg
+        self._bank = None
         _check(lib().b2s_band_create(engine._h, C.byref(cfg), C.byref(self._h)))
+
+    def close(self):
+        """b2s_band_destroy: an attached bank is detached first and stays usable on its own."""
+        super().close()
+        if self._bank is not None:
+            self._bank._band = None
+            self._bank = None
+
+    def attach_recorder_bank(self, bank: Optional["RecorderBank"]):
+        """b2s_band_attach_recorder_bank: every later push also runs `bank` over the pushed stream (one upload for both); None
+        detaches. The band keeps the bank alive while it is attached."""
+        _check(lib().b2s_band_attach_recorder_bank(self._h, bank._h if bank is not None else None))
+        if self._bank is not None:
+            self._bank._band = None
+        self._bank = bank
+        if bank is not None:
+            bank._band = weakref.ref(self)
 
     def set_stream(self, cuda_stream: int):
         _check(lib().b2s_band_set_stream(self._h, C.c_void_p(cuda_stream)))
@@ -613,8 +634,17 @@ class RecorderBank(_Handle):
         super().__init__(L.b2s_recorder_bank_destroy)
         self._e = engine
         self.sample_rate_hz, self.bandwidth_hz, self.n_channels, self.iq_format = sample_rate_hz, bandwidth_hz, n_channels, iq_format
+        self._band = None  # weak reference to the band this bank is attached to
         _check(L.b2s_recorder_bank_create(engine._h, sample_rate_hz, bandwidth_hz, iq_format, iq_scale, FLAG_IQ_ON_DEVICE if on_device else 0, n_channels,
                                           max_samples_per_push, C.byref(self._h)))
+
+    def close(self):
+        """b2s_recorder_bank_destroy: an attached bank is detached from its band first."""
+        super().close()
+        band = self._band() if self._band is not None else None
+        if band is not None and band._bank is self:
+            band._bank = None
+        self._band = None
 
     def start(self, channel: int, shift_hz: int):
         _check(lib().b2s_recorder_bank_start(self._h, channel, shift_hz))

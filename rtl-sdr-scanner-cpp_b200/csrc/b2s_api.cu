@@ -465,8 +465,22 @@ struct b2s_recorder_bank {
   std::vector<Stage> stages;
   DevBuf<unsigned char> carry_raw, staging;  // stage 0: the stream's newest raw samples (shared); host input staging
   DevBuf<signed char> d_out;                 // [n_ch][out_stride] int8 pairs
-  PinBuf<signed char> h_out;
+  // h_out[slot]: the host copy of d_out. A push launched from an asynchronous band leaves its host side pending; the next push uses the
+  // other slot, so its copy does not overwrite the output the pending push has not taken yet.
+  PinBuf<signed char> h_out[2];
+  Event out_ready[2];  // recorded after the device-to-host copy into h_out[slot] (pending pushes)
   size_t out_stride = 0;
+  // One push between its launch and its host side: the channels it ran, what each produced, and whether the output was copied back
+  struct Launched {
+    std::vector<int> rec;
+    std::vector<long long> produced;
+    long long most = 0;
+    int slot = 0;
+    bool fetch = false;
+  };
+  Launched pending;
+  bool has_pending = false;
+  b2s_band* band = nullptr;  // the band whose pushes feed this bank (b2s_band_attach_recorder_bank), or none
   struct Channel {
     bool recording = false, timed = false;  // timed: start_ms is set (the first push after start)
     unsigned long long phase_inc = 0;
@@ -573,28 +587,24 @@ int bank_create(b2s_engine* e, int32_t sample_rate_hz, int32_t bandwidth_hz, int
   k->out_stride = n_in;
   if ((rc = k->carry_raw.alloc(static_cast<size_t>(k->stages[0].hc) * k->raw_bytes()))) return rc;
   if ((rc = k->d_out.alloc(2 * k->out_stride * n_channels))) return rc;
-  if ((rc = k->h_out.alloc(2 * k->out_stride * n_channels))) return rc;
+  if ((rc = k->h_out[0].alloc(2 * k->out_stride * n_channels))) return rc;
   if (!k->on_device && (rc = k->staging.alloc(k->max_in * k->raw_bytes()))) return rc;
   out = std::move(k);
   return 0;
 }
 
-// The stream's next n_samples through every recording channel: one launch per stage (per kLaunchChannels channels), the channels'
-// int8 outputs back in one copy, one synchronise. Every check comes before the first copy or launch, so a refused push changes
-// nothing. n_out (optional): [n_ch] samples per channel; out_iq (optional): [n_ch][cap_samples] int8 pairs.
-int bank_push(b2s_recorder_bank* k, const void* iq, size_t n_samples, int64_t t0_ms, int8_t* out_iq, size_t cap_samples, bool check_cap, size_t* n_out,
-              const char* who) {
-  if (n_samples > k->max_in) return fail(B2S_E_INVALID, "%s: %zu samples exceed max_samples_per_push %zu", who, n_samples, k->max_in);
+// What a push of n_samples does: the recording channels (p.rec), each one's geometry in every stage ([channel][stage], the return value)
+// and output count (p.produced, p.most). Reads the channels' stream positions and changes nothing.
+std::vector<StageChan> bank_plan(const b2s_recorder_bank* k, size_t n_samples, b2s_recorder_bank::Launched& p) {
   const int n_st = static_cast<int>(k->stages.size());
-  std::vector<int> rec;
+  p.rec.clear();
   for (int i = 0; i < k->n_ch; ++i)
-    if (k->ch[i].recording) rec.push_back(i);
-  // every recording channel's geometry in every stage: [channel][stage]
-  std::vector<StageChan> geo(rec.size() * n_st);
-  std::vector<long long> produced(rec.size(), 0);
-  long long most = 0;
-  for (size_t i = 0; i < rec.size(); ++i) {
-    const auto& c = k->ch[rec[i]];
+    if (k->ch[i].recording) p.rec.push_back(i);
+  std::vector<StageChan> geo(p.rec.size() * n_st);
+  p.produced.assign(p.rec.size(), 0);
+  p.most = 0;
+  for (size_t i = 0; i < p.rec.size(); ++i) {
+    const auto& c = k->ch[p.rec[i]];
     long long seen = c.seen, n_in = static_cast<long long>(n_samples);
     for (int si = 0; si < n_st; ++si) {
       const auto& st = k->stages[si];
@@ -604,23 +614,23 @@ int bank_push(b2s_recorder_bank* k, const void* iq, size_t n_samples, int64_t t0
       g.n_in = static_cast<int>(n_in);
       g.n_out = static_cast<int>(stage_outputs(seen + n_in, st.interp, st.decim) - g.m0);
       g.phase_inc = si == 0 ? c.phase_inc : 0ull;
-      g.slot = rec[i];
+      g.slot = p.rec[i];
       seen = g.m0;
       n_in = g.n_out;
     }
-    produced[i] = n_in;
-    most = std::max(most, n_in);
+    p.produced[i] = n_in;
+    p.most = std::max(p.most, n_in);
   }
-  if (check_cap && static_cast<size_t>(most) > cap_samples) return fail(B2S_E_INVALID, "%s: %lld output samples, the buffer holds %zu", who, most, cap_samples);
-  if (n_out)
-    for (int i = 0; i < k->n_ch; ++i) n_out[i] = 0;
-  if (n_samples == 0) return 0;
-  CU(cudaSetDevice(k->engine->device));
-  const void* in = iq;
-  if (!k->on_device) {
-    CU(cudaMemcpyAsync(k->staging.p, iq, n_samples * k->raw_bytes(), cudaMemcpyHostToDevice, k->stream));
-    in = k->staging.p;
-  }
+  return geo;
+}
+
+// The device half of a push whose n_samples input samples are on the device at `in`: one launch per stage (per kLaunchChannels
+// channels), the carries, and (p.fetch) the copy of the channels' int8 outputs into h_out[p.slot], all on the bank's stream. Advances the
+// channels' stream positions. stage0_done (optional) is recorded once stage 0 and the raw carry no longer read `in`.
+int bank_launch(b2s_recorder_bank* k, const void* in, size_t n_samples, int64_t t0_ms, const std::vector<StageChan>& geo, const b2s_recorder_bank::Launched& p,
+                cudaEvent_t stage0_done) {
+  const int n_st = static_cast<int>(k->stages.size());
+  const std::vector<int>& rec = p.rec;
   const int raw_kind = k->iq_format == B2S_IQ_CS8 ? 0 : 1;
   for (int si = 0; si < n_st; ++si) {
     auto& st = k->stages[si];
@@ -668,28 +678,107 @@ int bank_push(b2s_recorder_bank* k, const void* iq, size_t n_samples, int64_t t0
       if (raw_kind == 0) k_shift_carry<short><<<1, 1024, st.hc * 2, k->stream>>>(static_cast<short*>(static_cast<void*>(k->carry_raw.p)), static_cast<const short*>(in), st.hc, n_samples);
       else k_shift_carry<double><<<1, 1024, st.hc * 8, k->stream>>>(static_cast<double*>(static_cast<void*>(k->carry_raw.p)), static_cast<const double*>(in), st.hc, n_samples);
       CU(cudaGetLastError());
+      if (stage0_done) CU(cudaEventRecord(stage0_done, k->stream));
     }
   }
-  const bool fetch = most > 0 && (out_iq || k->keep_chunks);
-  if (fetch) {
+  if (p.fetch) {
     const size_t rows = static_cast<size_t>(rec.back()) + 1, pitch = 2 * k->out_stride;
-    CU(cudaMemcpy2DAsync(k->h_out.p, pitch, k->d_out.p, pitch, 2 * static_cast<size_t>(most), rows, cudaMemcpyDeviceToHost, k->stream));
+    CU(cudaMemcpy2DAsync(k->h_out[p.slot].p, pitch, k->d_out.p, pitch, 2 * static_cast<size_t>(p.most), rows, cudaMemcpyDeviceToHost, k->stream));
   }
-  CU(cudaStreamSynchronize(k->stream));
-  for (size_t i = 0; i < rec.size(); ++i) {
-    auto& c = k->ch[rec[i]];
-    const size_t bytes = 2 * static_cast<size_t>(produced[i]);
-    const int8_t* src = reinterpret_cast<const int8_t*>(k->h_out.p) + 2 * k->out_stride * rec[i];
-    if (fetch && out_iq) std::memcpy(out_iq + 2 * cap_samples * rec[i], src, bytes);
-    if (fetch && k->keep_chunks) c.hold(src, bytes, 2 * static_cast<size_t>(k->chunk_samples));
+  for (int r : rec) {
+    auto& c = k->ch[r];
     if (!c.timed) {
       c.timed = true;
       c.start_ms = t0_ms;
     }
     c.seen += static_cast<long long>(n_samples);
-    if (n_out) n_out[rec[i]] = static_cast<size_t>(produced[i]);
   }
   return 0;
+}
+
+// The host half of a launched push, once its output copy has completed: each channel keeps its samples as chunks, and a direct push
+// also hands them to the caller (out_iq, n_out).
+void bank_take(b2s_recorder_bank* k, const b2s_recorder_bank::Launched& p, int8_t* out_iq, size_t cap_samples, size_t* n_out) {
+  for (size_t i = 0; i < p.rec.size(); ++i) {
+    auto& c = k->ch[p.rec[i]];
+    const size_t bytes = 2 * static_cast<size_t>(p.produced[i]);
+    const int8_t* src = reinterpret_cast<const int8_t*>(k->h_out[p.slot].p) + 2 * k->out_stride * p.rec[i];
+    if (p.fetch && out_iq) std::memcpy(out_iq + 2 * cap_samples * p.rec[i], src, bytes);
+    if (p.fetch && k->keep_chunks) c.hold(src, bytes, 2 * static_cast<size_t>(k->chunk_samples));
+    if (n_out) n_out[p.rec[i]] = static_cast<size_t>(p.produced[i]);
+  }
+}
+
+// The host side of the push that a band left pending (an asynchronous band's latest piece), if there is one
+int bank_settle(b2s_recorder_bank* k) {
+  if (!k->has_pending) return 0;
+  CU(cudaSetDevice(k->engine->device));
+  CU(cudaEventSynchronize(k->out_ready[k->pending.slot]));
+  k->has_pending = false;
+  bank_take(k, k->pending, nullptr, 0, nullptr);
+  return 0;
+}
+
+// The stream's next n_samples through every recording channel: one launch per stage (per kLaunchChannels channels), the channels'
+// int8 outputs back in one copy, one synchronise. Every check comes before the first copy or launch, so a refused push changes
+// nothing. n_out (optional): [n_ch] samples per channel; out_iq (optional): [n_ch][cap_samples] int8 pairs.
+int bank_push(b2s_recorder_bank* k, const void* iq, size_t n_samples, int64_t t0_ms, int8_t* out_iq, size_t cap_samples, bool check_cap, size_t* n_out,
+              const char* who) {
+  int rc = bank_settle(k);
+  if (rc) return rc;
+  if (n_samples > k->max_in) return fail(B2S_E_INVALID, "%s: %zu samples exceed max_samples_per_push %zu", who, n_samples, k->max_in);
+  b2s_recorder_bank::Launched p;
+  const std::vector<StageChan> geo = bank_plan(k, n_samples, p);
+  if (check_cap && static_cast<size_t>(p.most) > cap_samples) return fail(B2S_E_INVALID, "%s: %lld output samples, the buffer holds %zu", who, p.most, cap_samples);
+  if (n_out)
+    for (int i = 0; i < k->n_ch; ++i) n_out[i] = 0;
+  if (n_samples == 0) return 0;
+  CU(cudaSetDevice(k->engine->device));
+  const void* in = iq;
+  if (!k->on_device) {
+    CU(cudaMemcpyAsync(k->staging.p, iq, n_samples * k->raw_bytes(), cudaMemcpyHostToDevice, k->stream));
+    in = k->staging.p;
+  }
+  p.fetch = p.most > 0 && (out_iq || k->keep_chunks);
+  if ((rc = bank_launch(k, in, n_samples, t0_ms, geo, p, nullptr))) return rc;
+  CU(cudaStreamSynchronize(k->stream));
+  bank_take(k, p, out_iq, cap_samples, n_out);
+  return 0;
+}
+
+// One piece of an attached band's push through the bank: the n_samples already on the device at `in`, read once `ready` (an event of
+// the band's) has fired. The piece stays pending (its host side is done by bank_settle); the push pending before it is settled here,
+// after this one is launched into the other output slot, so that the bank's kernels of consecutive pieces follow each other without a
+// host wait in between.
+int bank_feed(b2s_recorder_bank* k, const void* in, size_t n_samples, int64_t t0_ms, cudaEvent_t ready, cudaEvent_t stage0_done) {
+  int rc = 0;
+  // with one output slot (a bank that has only fed synchronous bands) the pending piece, left by a push that failed, is settled first
+  if (k->has_pending && !k->h_out[1].p && (rc = bank_settle(k))) return rc;
+  b2s_recorder_bank::Launched p;
+  const std::vector<StageChan> geo = bank_plan(k, n_samples, p);
+  p.slot = k->has_pending ? k->pending.slot ^ 1 : 0;
+  p.fetch = p.most > 0;
+  CU(cudaStreamWaitEvent(k->stream, ready, 0));
+  rc = bank_launch(k, in, n_samples, t0_ms, geo, p, stage0_done);
+  if (rc) return rc;
+  CU(cudaEventRecord(k->out_ready[p.slot], k->stream));
+  if ((rc = bank_settle(k))) return rc;
+  k->pending = std::move(p);
+  k->has_pending = true;
+  return 0;
+}
+
+// Detach the band's bank (b->mutex held): the band's outstanding pushes are drained and the bank's last push settled, so that neither
+// object refers to the other afterwards. The bank keeps its stream position. Detaches even when draining reports an earlier error,
+// which it then returns.
+int band_detach(b2s_band* b) {
+  if (!b->bank) return 0;
+  int rc = b->drain();
+  const int rc2 = bank_settle(b->bank);
+  b->bank->band = nullptr;
+  b->bank = nullptr;
+  b->d_whole = DevBuf<unsigned char>();
+  return rc ? rc : rc2;
 }
 
 }  // namespace
@@ -798,8 +887,39 @@ int b2s_band_create(b2s_engine* e, const b2s_band_config* cfg, b2s_band** out) {
 int b2s_band_destroy(b2s_band* b) {
   if (b) {
     cudaSetDevice(b->engine->device);
+    {
+      std::lock_guard<std::mutex> lock(b->mutex);
+      band_detach(b);  // the bank continues on its own
+    }
     delete b;
   }
+  return 0;
+}
+
+int b2s_band_attach_recorder_bank(b2s_band* b, b2s_recorder_bank* k) {
+  if (!b) return fail(B2S_E_INVALID, "NULL band");
+  std::lock_guard<std::mutex> lock(b->mutex);
+  CU(cudaSetDevice(b->engine->device));
+  if (!k) return band_detach(b);
+  if (b->bank) return fail(B2S_E_INVALID, "b2s_band_attach_recorder_bank: the band already has a recorder bank (detach it first)");
+  if (k->band) return fail(B2S_E_INVALID, "b2s_band_attach_recorder_bank: the recorder bank is attached to a band");
+  if (k->engine != b->engine) return fail(B2S_E_INVALID, "b2s_band_attach_recorder_bank: the recorder bank belongs to another engine");
+  if (k->sample_rate != b->cfg.sample_rate_hz || k->iq_format != b->cfg.iq_format || k->iq_scale != b->cfg.iq_scale)
+    return fail(B2S_E_INVALID, "b2s_band_attach_recorder_bank: the recorder bank's sample rate, iq_format or iq_scale differs from the band's");
+  const size_t stride = static_cast<size_t>(b->cfg.frame_stride_samples), need = static_cast<size_t>(b->max_frames) * stride;
+  if (k->max_in < need)
+    return fail(B2S_E_INVALID, "b2s_band_attach_recorder_bank: max_samples_per_push %zu is below max_frames_per_push x frame_stride_samples = %zu", k->max_in, need);
+  // everything the attachment needs is allocated before either object changes
+  DevBuf<unsigned char> whole;
+  int rc = 0;
+  if (!(b->cfg.flags & B2S_FLAG_IQ_ON_DEVICE) && !b->async_mode && (rc = whole.alloc(need * k->raw_bytes()))) return rc;
+  if (b->async_mode && (rc = k->h_out[1].alloc(k->h_out[0].n))) return rc;  // its latest piece is still pending when the next one launches
+  for (auto* e : {&b->bank_prev_use[0], &b->bank_prev_use[1], &b->push_ready, &b->bank_read, &k->out_ready[0], &k->out_ready[1]}) {
+    if (!*e) CU(cudaEventCreateWithFlags(&e->h, cudaEventDisableTiming));
+  }
+  b->d_whole = std::move(whole);
+  b->bank = k;
+  k->band = b;
   return 0;
 }
 int b2s_band_set_stream(b2s_band* b, void* cuda_stream) {
@@ -830,14 +950,30 @@ int b2s_band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, d
   const size_t bytes_per_sample = b->cfg.iq_format == B2S_IQ_CS8 ? 2 : 8;
   const size_t stride_bytes = static_cast<size_t>(b->cfg.frame_stride_samples) * bytes_per_sample;
   const bool on_device = (b->cfg.flags & B2S_FLAG_IQ_ON_DEVICE) != 0;
+  // An attached bank reads the push as pieces of up to max_frames frames (frame_stride_samples each), piece j stamped like frame
+  // j * max_frames. A synchronous band settles each piece before it moves on; an asynchronous one leaves the newest piece pending.
+  const size_t stride = static_cast<size_t>(b->cfg.frame_stride_samples);
+  auto settle_if_sync = [&]() { return b->bank && !b->async_mode ? bank_settle(b->bank) : 0; };
+  if (b->bank && n_frames == 0) {
+    const int rc = bank_settle(b->bank);
+    if (rc) return rc;
+  }
   if (on_device) {
-    for (size_t done = 0; done < n_frames;) {
+    if (b->bank) CU(cudaEventRecord(b->push_ready, b->stream));  // the bank reads the caller's buffer no earlier than K1 could
+    int rc = 0;
+    for (size_t done = 0; done < n_frames && !rc;) {
       const size_t chunk = std::min(n_frames - done, static_cast<size_t>(b->max_frames));
-      int rc = b->push_chunk(static_cast<const char*>(iq) + done * stride_bytes, chunk, t0_ms, frame_period_ms, done, out);
-      if (rc) return rc;
+      const char* piece = static_cast<const char*>(iq) + done * stride_bytes;
+      rc = b->bank ? bank_feed(b->bank, piece, chunk * stride, host::frame_time(t0_ms, frame_period_ms, done), b->push_ready, b->bank_read) : 0;
+      if (!rc) rc = b->push_chunk(piece, chunk, t0_ms, frame_period_ms, done, out);
+      if (!rc) rc = settle_if_sync();
       done += chunk;
     }
-    return 0;
+    // The caller may reuse `iq` in the band's stream order once the call returns, also when it failed: what follows on `stream` waits
+    // for the bank's reads of it (the bank's stream is in order, so its last piece's stage 0 comes after every earlier one's), as it
+    // follows K1. The wait comes after the push's own kernels, which therefore never wait for the bank.
+    if (b->bank) CU(cudaStreamWaitEvent(b->stream, b->bank_read, 0));
+    return rc;
   }
   // Host input: the push is cut into pipeline chunks; the host->device copy of chunk i+1 runs on a second stream
   // while chunk i is in the kernels / tracker (double-buffered staging), so PCIe time hides behind compute (or vice versa).
@@ -849,6 +985,35 @@ int b2s_band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, d
     CU(cudaEventCreateWithFlags(&b->copy_done[0].h, cudaEventDisableTiming));
     CU(cudaEventCreateWithFlags(&b->copy_done[1].h, cudaEventDisableTiming));
   }
+  if (b->bank && !b->async_mode) {
+    // Each piece is staged whole in d_whole: its pipeline chunks are copied to their offsets, and the bank is launched on the piece as
+    // soon as the copy of its last chunk has been issued, so that its kernels run beside the band's chunks.
+    unsigned char* whole = b->d_whole.p;
+    for (size_t p0 = 0; p0 < n_frames; p0 += b->max_frames) {
+      const size_t piece = std::min(n_frames - p0, static_cast<size_t>(b->max_frames));
+      const size_t part = piece >= 512 ? (piece + 3) / 4 : piece;
+      auto copy_part = [&](size_t off, int slot) -> int {
+        const size_t bytes = std::min(part, piece - off) * stride_bytes;
+        CU(cudaMemcpyAsync(whole + off * stride_bytes, static_cast<const char*>(iq) + (p0 + off) * stride_bytes, bytes, cudaMemcpyHostToDevice, b->copy_stream));
+        CU(cudaEventRecord(b->copy_done[slot], b->copy_stream));
+        b->prof.h2d_bytes += bytes;
+        if (off + part < piece) return 0;
+        return bank_feed(b->bank, whole, piece * stride, host::frame_time(t0_ms, frame_period_ms, p0), b->copy_done[slot], b->bank_read);
+      };
+      // d_whole is overwritten only after the bank has read the previous piece (still pending if the push that fed it failed)
+      CU(cudaStreamWaitEvent(b->copy_stream, b->bank_read, 0));
+      int rc = copy_part(0, 0);
+      if (rc) return rc;
+      int slot = 0;
+      for (size_t off = 0; off < piece; off += part, slot ^= 1) {
+        CU(cudaStreamWaitEvent(b->stream, b->copy_done[slot], 0));
+        if (off + part < piece && (rc = copy_part(off + part, slot ^ 1))) return rc;
+        if ((rc = b->push_chunk(whole + off * stride_bytes, std::min(part, piece - off), t0_ms, frame_period_ms, p0 + off, out))) return rc;
+      }
+      if ((rc = bank_settle(b->bank))) return rc;
+    }
+    return 0;
+  }
   const size_t buf_bytes = pipe * stride_bytes;
   for (int i = 0; i < 2; ++i) {
     int rc = b->d_iq[i].alloc(buf_bytes);
@@ -857,7 +1022,8 @@ int b2s_band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, d
   auto chunk_len = [&](size_t done) { return std::min(n_frames - done, pipe); };
   auto start_copy = [&](size_t done, int slot) -> int {
     const size_t chunk = chunk_len(done);
-    const size_t bytes = (chunk - 1) * stride_bytes + static_cast<size_t>(b->cfg.fft_size) * bytes_per_sample;  // the last frame needs N samples only
+    // the last frame needs N samples only, unless a bank reads the whole stream
+    const size_t bytes = b->bank ? chunk * stride_bytes : (chunk - 1) * stride_bytes + static_cast<size_t>(b->cfg.fft_size) * bytes_per_sample;
     CU(cudaMemcpyAsync(b->d_iq[slot].p, static_cast<const char*>(iq) + done * stride_bytes, bytes, cudaMemcpyHostToDevice, b->copy_stream));
     CU(cudaEventRecord(b->copy_done[slot], b->copy_stream));
     b->prof.h2d_bytes += bytes;
@@ -870,9 +1036,13 @@ int b2s_band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, d
       const size_t chunk = chunk_len(done);
       const int slot = b->iq_slot;
       CU(cudaStreamWaitEvent(b->copy_stream, b->iq_prev_use[slot], 0));
+      if (b->bank) CU(cudaStreamWaitEvent(b->copy_stream, b->bank_prev_use[slot], 0));  // and the bank's stage 0 that read it
       int rc = start_copy(done, slot);
       if (rc) return rc;
       CU(cudaStreamWaitEvent(b->stream, b->copy_done[slot], 0));
+      // a chunk is a whole piece here (pipe = max_frames when the push is longer)
+      if (b->bank && (rc = bank_feed(b->bank, b->d_iq[slot].p, chunk * stride, host::frame_time(t0_ms, frame_period_ms, done), b->copy_done[slot], b->bank_prev_use[slot])))
+        return rc;
       rc = b->push_chunk(b->d_iq[slot].p, chunk, t0_ms, frame_period_ms, done, nullptr);
       if (rc) return rc;
       CU(cudaEventRecord(b->iq_prev_use[slot], b->stream));  // K1 (and the rest) of this chunk: the buffer may be overwritten after it
@@ -908,6 +1078,7 @@ int b2s_band_sync(b2s_band* b, b2s_result* out) {
   CU(cudaSetDevice(b->engine->device));
   int rc = b->drain();
   if (rc) return rc;
+  if (b->bank && (rc = bank_settle(b->bank))) return rc;
   if (out) {
     out->n_transmissions_total = static_cast<int32_t>(b->mailbox.size());
     out->n_transmissions = std::min<int32_t>(out->n_transmissions_total, B2S_MAX_TX);
@@ -1290,18 +1461,26 @@ int b2s_recorder_bank_create(b2s_engine* e, int32_t sample_rate_hz, int32_t band
 int b2s_recorder_bank_destroy(b2s_recorder_bank* k) {
   if (k) {
     cudaSetDevice(k->engine->device);
+    if (k->band) {  // detach first: the band goes on without the bank
+      std::lock_guard<std::mutex> lock(k->band->mutex);
+      band_detach(k->band);
+    }
     delete k;
   }
   return 0;
 }
 int b2s_recorder_bank_start(b2s_recorder_bank* k, int channel, int32_t shift_hz) {
   if (!k || channel < 0 || channel >= k->n_ch) return fail(B2S_E_INVALID, "b2s_recorder_bank_start: bad channel");
+  const int rc = bank_settle(k);  // a push an asynchronous band left pending belongs to the recording as it was
+  if (rc) return rc;
   if (k->ch[channel].recording) return fail(B2S_E_STATE, "b2s_recorder_bank_start: channel %d is already recording", channel);
   start_channel(k->ch[channel], rotator_phase_inc(shift_hz, k->sample_rate));
   return 0;
 }
 int b2s_recorder_bank_stop(b2s_recorder_bank* k, int channel) {
   if (!k || channel < 0 || channel >= k->n_ch) return fail(B2S_E_INVALID, "b2s_recorder_bank_stop: bad channel");
+  const int rc = bank_settle(k);
+  if (rc) return rc;
   auto& c = k->ch[channel];
   if (!c.recording) return fail(B2S_E_STATE, "b2s_recorder_bank_stop: channel %d is not recording", channel);
   c.recording = false;
@@ -1316,6 +1495,8 @@ int b2s_recorder_bank_push(b2s_recorder_bank* k, const void* iq, size_t n_sample
 // last sample arrives on the injected clock: start_ms + floor((j + 1) * chunk_samples * 1000 / bandwidth + 0.5)
 int b2s_recorder_bank_flush(b2s_recorder_bank* k, int channel, int8_t* chunks, int64_t* times_ms, int cap, int consume, int* count, int* chunk_samples) {
   if (!k || channel < 0 || channel >= k->n_ch || cap < 0) return fail(B2S_E_INVALID, "b2s_recorder_bank_flush: bad argument");
+  const int rc = bank_settle(k);
+  if (rc) return rc;
   auto& c = k->ch[channel];
   const size_t chunk_bytes = 2 * static_cast<size_t>(k->chunk_samples);
   const int avail = static_cast<int>(std::min<size_t>(c.chunks.size(), std::numeric_limits<int>::max()));

@@ -92,6 +92,15 @@ struct b2s_band : public DeviceQueries {
   DevBuf<TrackState> d_state;     // the signal map (device resident; tracker.signals mirrors it only inside a host-tracked push)
   Event copy_done[2], iq_prev_use[2];
   int iq_slot = 0;
+  // recorder bank fed from this band's pushes (b2s_band_attach_recorder_bank). While one is attached, host input is staged with every
+  // frame's whole stride: the synchronous path stages a whole piece of up to max_frames frames in d_whole (pipeline chunks at their
+  // offsets), the asynchronous path reads d_iq, whose copy also waits for bank_prev_use[slot] (the bank's stage 0 of the last push that
+  // read the buffer). push_ready marks, on `stream`, the start of a push with device input; the bank's stream waits for it. bank_read
+  // marks, on the bank's stream, the end of its reads of the last piece from d_whole or the caller's device buffer: the next copy into
+  // d_whole, and with device input the band's stream after the piece's kernels, wait for it.
+  b2s_recorder_bank* bank = nullptr;
+  DevBuf<unsigned char> d_whole;
+  Event bank_prev_use[2], push_ready, bank_read;
   int max_frames = 0;
   int slot_capacity = 0;  // detection entries per frame
   int detect_bins = kDetectBinsPerCta;  // bins per K2 CTA (DetectArgs::bins_per_cta)
