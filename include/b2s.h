@@ -37,14 +37,13 @@ extern "C" {
 #define B2S_E_CUDA (-2)      /* CUDA runtime error (sticky errors: destroy and re-create the engine) */
 #define B2S_E_NOMEM (-3)
 #define B2S_E_OVERFLOW (-4)  /* a frame had more detection entries than detect_capacity: the push completed on truncated lists (state
-                                stays consistent), the capacity grows before the next push; or more live signals than the engine tracks */
+                                stays consistent), the capacity grows before the next push */
 #define B2S_E_STATE (-5)
 
 #define B2S_MAX_IGNORED 16
 #define B2S_MAX_TX 64        /* transmissions held INSIDE b2s_result; the signal map itself is not limited to this:
                                 n_transmissions_total reports the real count and b2s_band_get_transmissions returns the whole list.
-                                The device-resident map holds up to 256 live signals per band (the reference's std::map is
-                                unbounded); beyond that a push fails with B2S_E_OVERFLOW instead of dropping signals */
+                                Like the reference's std::map, the device-resident map has no cap on live signals */
 
 #define B2S_IQ_CS8 0         /* interleaved int8 I,Q (help_structures.h:17 SimpleComplex) */
 #define B2S_IQ_CF32 1        /* interleaved float I,Q (what SdrSource delivers, sdr_source.cpp:52) */
@@ -170,8 +169,8 @@ typedef struct b2s_profile {
   int64_t h2d_bytes, d2h_bytes; /* bytes moved by b2s_band_push itself */
   /* load balance of K2 (one CTA per 128 bins): per-CTA run time in ms, median and slowest, summed over launches */
   double detect_cta_median_ms, detect_cta_max_ms;
-  double track_ms;           /* K4 k_runs + k_track: the signal map on the device (runs beside the next push's K1) */
-  int64_t track_launches;
+  double track_ms;           /* K4 k_track + k_track_wide: the signal map on the device (runs beside the next push's K1) */
+  int64_t track_launches;    /* K4 launches that ran a push: one per device-tracked push, two when k_track left it to k_track_wide */
   int64_t track_evals, track_events, track_best_index;  /* K4 work counters: block evaluations, event frames replayed, getBestIndex calls */
 } b2s_profile;
 int b2s_band_set_profiling(b2s_band* b, int enable); /* 0 off, 1 kernel times and byte counts, 2 also K2 per-CTA run times */

@@ -1201,15 +1201,16 @@ int b2s_band_get_signals(b2s_band* b, int32_t* keys, int64_t* first, int64_t* la
   CU(cudaSetDevice(b->engine->device));
   int rc = b->drain();
   if (rc) return rc;
-  std::vector<TrackState> h(1);  // the map is device resident (K4)
-  if ((rc = b->download_state(h[0]))) return rc;
-  for (int i = 0; i < h[0].n && i < cap; ++i) {
-    if (keys) keys[i] = h[0].key[i];
-    if (first) first[i] = h[0].first[i];
-    if (last) last[i] = h[0].last[i];
-    if (power) power[i] = h[0].power[i];
+  b2s_band::HostMap h;  // the map is device resident (K4)
+  if ((rc = b->download_state(h))) return rc;
+  const int n = static_cast<int>(h.key.size());
+  for (int i = 0; i < n && i < cap; ++i) {
+    if (keys) keys[i] = h.key[i];
+    if (first) first[i] = h.first[i];
+    if (last) last[i] = h.last[i];
+    if (power) power[i] = h.power[i];
   }
-  *count = h[0].n;
+  *count = n;
   return 0;
 }
 

@@ -54,6 +54,7 @@ struct PushSlot {
   DevBuf<float> box_last;
   DevBuf<int> run_lo, run_hi, run_count;  // RunFold arrays of the chunk
   DevBuf<TrackResult> d_result;
+  DevBuf<b2s_transmission> d_tx;  // [N] the push's whole sorted list (TrackArgs::tx)
   PinBuf<TrackResult> h_result;
   Event sorted_done, tev[2];
   bool host_track = false;  // this chunk's bookkeeping runs on the host (the caller asked for every frame's list)
@@ -89,7 +90,14 @@ struct b2s_band : public DeviceQueries {
   Stream own_stream, finish_stream, copy_stream;
   Stream track_stream;            // K4 of push k runs here, beside K1 of push k+1 on `stream`
   cudaStream_t stream = nullptr;  // own_stream, or the caller's stream (b2s_band_set_stream)
-  DevBuf<TrackState> d_state;     // the signal map (device resident; tracker.signals mirrors it only inside a host-tracked push)
+  // the signal map (device resident; tracker.signals mirrors it only inside a host-tracked push): the live count and arrays of
+  // N entries (TrackMap), and k_track_wide's hit words and sort keys. About 180 B per bin with the slots' d_tx.
+  DevBuf<int> d_map_n, d_map_key;
+  DevBuf<long long> d_map_first, d_map_last;
+  DevBuf<float> d_map_power;
+  DevBuf<unsigned int> d_track_hit;
+  DevBuf<unsigned long long> d_track_sort;
+  TrackMap track_map() { return TrackMap{d_map_n.p, d_map_key.p, d_map_first.p, d_map_last.p, d_map_power.p}; }
   Event copy_done[2], iq_prev_use[2];
   int iq_slot = 0;
   // recorder bank fed from this band's pushes (b2s_band_attach_recorder_bank). While one is attached, host input is staged with every
@@ -362,10 +370,17 @@ struct b2s_band : public DeviceQueries {
       if ((rc = s.run_hi.alloc(static_cast<size_t>(2 * kRunCap) * max_frames))) return rc;
       if ((rc = s.run_count.alloc(static_cast<size_t>(2) * max_frames))) return rc;
       if ((rc = s.d_result.alloc(1))) return rc;
+      if ((rc = s.d_tx.alloc(n))) return rc;
       if ((rc = s.h_result.alloc(1))) return rc;
     }
-    if ((rc = d_state.alloc(1))) return rc;
-    CU(cudaMemset(d_state.p, 0, sizeof(TrackState)));
+    if ((rc = d_map_n.alloc(1)) || (rc = d_map_key.alloc(n)) || (rc = d_map_first.alloc(n)) || (rc = d_map_last.alloc(n)) || (rc = d_map_power.alloc(n))) return rc;
+    CU(cudaMemset(d_map_n.p, 0, sizeof(int)));
+    if ((rc = d_track_hit.alloc(n * kTrackWords))) return rc;
+    {
+      size_t sort_cap = 2;
+      while (sort_cap < n) sort_cap <<= 1;
+      if ((rc = d_track_sort.alloc(sort_cap))) return rc;
+    }
     if ((rc = d_sum[0].alloc(n))) return rc;
     if ((rc = d_sum[1].alloc(n))) return rc;
     for (auto& r : d_ring) {
@@ -442,33 +457,51 @@ struct b2s_band : public DeviceQueries {
     tp.max_time = p.max_time;
     return tp;
   }
-  int download_state(TrackState& h) {
+  struct HostMap {
+    std::vector<int> key;
+    std::vector<long long> first, last;
+    std::vector<float> power;
+  };
+  int download_state(HostMap& h) {
     CU(cudaStreamSynchronize(track_stream));
-    CU(cudaMemcpy(&h, d_state.p, sizeof(TrackState), cudaMemcpyDeviceToHost));
+    int count = 0;
+    CU(cudaMemcpy(&count, d_map_n.p, sizeof(int), cudaMemcpyDeviceToHost));
+    h.key.resize(count);
+    h.first.resize(count);
+    h.last.resize(count);
+    h.power.resize(count);
+    if (count > 0) {
+      CU(cudaMemcpy(h.key.data(), d_map_key.p, sizeof(int) * count, cudaMemcpyDeviceToHost));
+      CU(cudaMemcpy(h.first.data(), d_map_first.p, sizeof(long long) * count, cudaMemcpyDeviceToHost));
+      CU(cudaMemcpy(h.last.data(), d_map_last.p, sizeof(long long) * count, cudaMemcpyDeviceToHost));
+      CU(cudaMemcpy(h.power.data(), d_map_power.p, sizeof(float) * count, cudaMemcpyDeviceToHost));
+    }
     return 0;
   }
   int state_to_host_tracker() {
-    std::vector<TrackState> h(1);
-    int rc = download_state(h[0]);
+    HostMap h;
+    int rc = download_state(h);
     if (rc) return rc;
     tracker.signals.clear();
-    for (int i = 0; i < h[0].n; ++i) tracker.signals[h[0].key[i]] = TrackedSignal{h[0].first[i], h[0].last[i], h[0].power[i], -1};
+    for (size_t i = 0; i < h.key.size(); ++i) tracker.signals[h.key[i]] = TrackedSignal{h.first[i], h.last[i], h.power[i], -1};
     return 0;
   }
   int host_tracker_to_state() {
-    if (tracker.signals.size() > static_cast<size_t>(kMaxSignals)) return fail(B2S_E_OVERFLOW, "%zu live signals; the engine tracks at most %d per band", tracker.signals.size(), kMaxSignals);
-    std::vector<TrackState> h(1);
-    std::memset(&h[0], 0, sizeof(TrackState));
-    int i = 0;
+    HostMap h;
     for (const auto& kv : tracker.signals) {
-      h[0].key[i] = kv.first;
-      h[0].first[i] = kv.second.first;
-      h[0].last[i] = kv.second.last;
-      h[0].power[i] = kv.second.power;
-      ++i;
+      h.key.push_back(kv.first);
+      h.first.push_back(kv.second.first);
+      h.last.push_back(kv.second.last);
+      h.power.push_back(kv.second.power);
     }
-    h[0].n = i;
-    CU(cudaMemcpy(d_state.p, &h[0], sizeof(TrackState), cudaMemcpyHostToDevice));
+    const int count = static_cast<int>(h.key.size());
+    if (count > 0) {
+      CU(cudaMemcpy(d_map_key.p, h.key.data(), sizeof(int) * count, cudaMemcpyHostToDevice));
+      CU(cudaMemcpy(d_map_first.p, h.first.data(), sizeof(long long) * count, cudaMemcpyHostToDevice));
+      CU(cudaMemcpy(d_map_last.p, h.last.data(), sizeof(long long) * count, cudaMemcpyHostToDevice));
+      CU(cudaMemcpy(d_map_power.p, h.power.data(), sizeof(float) * count, cudaMemcpyHostToDevice));
+    }
+    CU(cudaMemcpy(d_map_n.p, &count, sizeof(int), cudaMemcpyHostToDevice));
     return 0;
   }
 
@@ -488,7 +521,7 @@ struct b2s_band : public DeviceQueries {
   // behind the pushes already in flight (Scanner hops every 500 ms, scanner.cpp:46-60: a hop must not drain the pipeline).
   int reset_buffers() {
     tracker.reset();
-    CU(cudaMemsetAsync(d_state.p, 0, sizeof(TrackState), track_stream));  // behind the K4 of every earlier push, before the next one's
+    CU(cudaMemsetAsync(d_map_n.p, 0, sizeof(int), track_stream));  // behind the K4 of every earlier push, before the next one's
     {
       std::lock_guard<std::mutex> lk(qmutex);
       reset_epoch += 1;  // a chunk enqueued before this moment must not publish its (pre-reset) list afterwards
@@ -851,10 +884,18 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
     ta.noise_samples = da.noise_samples;
     ta.learn_frames = da.learn_frames;
     ta.ring_before = d_ring[ring_in].p;
-    ta.state = d_state.p;
+    ta.state = track_map();
     ta.result = s.d_result.p;
-    auto* track = run_len_bits(cfg.fft_size) == 14 ? k_track<14> : k_track<12>;
+    ta.tx = s.d_tx.p;
+    ta.hit = d_track_hit.p;
+    ta.sort_keys = d_track_sort.p;
+    // k_track runs the push unless it would pass its shared tables; then it leaves the map untouched and sets the result's
+    // hand-off flag, and k_track_wide, always enqueued behind it, runs the push from the same map. Otherwise k_track_wide exits.
+    const bool len14 = run_len_bits(cfg.fft_size) == 14;
+    auto* track = len14 ? k_track<14> : k_track<12>;
+    auto* wide = len14 ? k_track_wide<14> : k_track_wide<12>;
     if ((rc = prepare_kernel(engine, track, kTrackThreads, sizeof(TrackShared), nullptr))) return rc;
+    if ((rc = prepare_kernel(engine, wide, kTrackThreads, sizeof(TrackWideShared), nullptr))) return rc;
     if (profiling) {
       for (auto& e : s.tev) {
         if (!e) CU(cudaEventCreate(&e.h));
@@ -863,9 +904,11 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
     }
     track<<<1, kTrackThreads, sizeof(TrackShared), track_stream>>>(ta);
     CU(cudaGetLastError());
+    wide<<<1, kTrackThreads, sizeof(TrackWideShared), track_stream>>>(ta);
+    CU(cudaGetLastError());
     if (profiling) CU(cudaEventRecord(s.tev[1], track_stream));
     // the result header and the first B2S_MAX_TX transmissions (the rest, if any, is fetched by the finish half)
-    CU(cudaMemcpyAsync(s.h_result.p, s.d_result.p, offsetof(TrackResult, tx) + sizeof(b2s_transmission) * B2S_MAX_TX, cudaMemcpyDeviceToHost, track_stream));
+    CU(cudaMemcpyAsync(s.h_result.p, s.d_result.p, sizeof(TrackResult), cudaMemcpyDeviceToHost, track_stream));
     CU(cudaEventRecord(s.gpu_done, track_stream));
     prof.track_launches += 1;
   } else {
@@ -918,9 +961,8 @@ int b2s_band::finish_chunk(PushSlot& s) {
     if (st != stream) CU(cudaStreamWaitEvent(st, s.gpu_done, 0));
     const auto host_t0 = std::chrono::steady_clock::now();
     const TrackResult& r = *s.h_result.p;
-    prof.d2h_bytes += offsetof(TrackResult, tx) + sizeof(b2s_transmission) * B2S_MAX_TX;
-    if (r.error & 1) return fail(B2S_E_OVERFLOW, "more than %d live signals in one band", kMaxSignals);
-    if (r.error & 2) return fail(B2S_E_OVERFLOW, "more than %d start-level candidates in one frame", kMaxCand);
+    prof.d2h_bytes += sizeof(TrackResult);
+    prof.track_launches += r.handoff;  // k_track_wide ran the push
     n_entries = r.n_entries;
     worst_count = r.max_count;
     prof.track_evals += r.n_evals;
@@ -930,7 +972,7 @@ int b2s_band::finish_chunk(PushSlot& s) {
     std::vector<b2s_transmission> list(r.n_tx);
     std::memcpy(list.data(), r.tx, sizeof(b2s_transmission) * std::min(r.n_tx, B2S_MAX_TX));
     if (r.n_tx > B2S_MAX_TX) {  // rare: the tail of a long list
-      CU(cudaMemcpyAsync(list.data() + B2S_MAX_TX, s.d_result.p->tx + B2S_MAX_TX, sizeof(b2s_transmission) * (r.n_tx - B2S_MAX_TX), cudaMemcpyDeviceToHost, st));
+      CU(cudaMemcpyAsync(list.data() + B2S_MAX_TX, s.d_tx.p + B2S_MAX_TX, sizeof(b2s_transmission) * (r.n_tx - B2S_MAX_TX), cudaMemcpyDeviceToHost, st));
       CU(cudaStreamSynchronize(st));
       prof.d2h_bytes += sizeof(b2s_transmission) * (r.n_tx - B2S_MAX_TX);
     }
