@@ -192,6 +192,34 @@ int b2s_band_get_transmissions(b2s_band* b, b2s_transmission* out, int cap, int*
 /* live signals (the std::map<Index, Signal> of transmission.h:49) */
 int b2s_band_get_signals(b2s_band* b, int32_t* keys, int64_t* first_ms, int64_t* last_ms, float* power, int cap, int* count);
 
+/* ---- signal event log: every change of the signal map, in the order Transmission::process makes them ----
+ * The mailbox shows the map after the last frame of a push only. The log (off by default) also keeps every insertion and erasure
+ * that happened in the frames of a push, so a transmission that starts and times out inside one push is still reported, and a
+ * start or stop comes with its frame. It replaces the Logger::info lines of transmission.cpp:75-80,101-107.
+ * Order: by frame; within a frame the STARTs in the order addSignals inserted them (strongest uncovered candidate first), then
+ * the STOPs in ascending key (the map order clearSignals walks). b2s_band_reset and b2s_band_set_center log nothing
+ * (resetBuffers is silent in the reference), and the events of frames pushed before them stay in the log. */
+#define B2S_EV_START 1  /* addSignals inserted the key (transmission.cpp:108) */
+#define B2S_EV_STOP 2   /* clearSignals erased it: isTimeout or isMaximalTime (transmission.cpp:73-81) */
+#define B2S_EV_LOST 3   /* `key` events of one device pass did not fit the device log (fft_size records per pass) and are missing at
+                           this point; frame and time_ms repeat the last event kept */
+typedef struct b2s_signal_event {
+  int32_t kind;      /* B2S_EV_* */
+  int32_t key;       /* map key (bin); for B2S_EV_LOST the number of events lost */
+  int32_t shift_hz;  /* getTunedFrequency(indexToShift(key), tuningStep): the value b2s_transmission.shift_hz carries */
+  int32_t reserved;
+  int64_t frame;     /* frames pushed to this band before the event's frame, counted from b2s_band_create (reset and retune do not
+                        restart it) */
+  int64_t time_ms;   /* the frame's injected clock */
+  int64_t first_ms;  /* Signal::m_firstDataTime (= time_ms for START) */
+  int64_t last_ms;   /* Signal::m_lastDataTime when erased (= time_ms for START) */
+} b2s_signal_event;
+/* enable != 0 turns the log on for the pushes after this call; turning it off drops nothing already logged */
+int b2s_band_set_event_log(b2s_band* b, int enable);
+/* events of the finished pushes, oldest first: up to `cap` are copied, *count is the number available; with consume != 0 the
+ * events copied out (and only those) are dropped from the log */
+int b2s_band_get_events(b2s_band* b, b2s_signal_event* out, int cap, int consume, int* count);
+
 /* ---- stand-alone operators (operator-level parity with the reference's unit tests) ---- */
 /* device-backed Averager with the reference's surface (averager.h:8-28) */
 typedef struct b2s_averager b2s_averager;
@@ -281,6 +309,9 @@ int b2s_host_transmission_reset(b2s_host_transmission* h); /* Transmission::rese
 double b2s_host_transmission_last_run_ms(b2s_host_transmission* h); /* wall time of the bookkeeping of the last push (measurement) */
 int b2s_host_transmission_push(b2s_host_transmission* h, const float* box_rows, const float* q_rows, int n_frames, int64_t t0_ms,
                                double frame_period_ms, int use_watch, int32_t* tx_count, b2s_transmission* tx);
+/* the tracker's signal event log (always kept here; conventions of b2s_band_get_events): `frame` counts the frames pushed since
+ * create */
+int b2s_host_transmission_get_events(b2s_host_transmission* h, b2s_signal_event* out, int cap, int consume, int* count);
 
 /* ---- wire formats of the reference's MQTT payloads (network/data_controller.cpp:27-57), little-endian, packed ----
  * so that rows / recordings produced here can be published to an unchanged sdr-hub. Both return 0 and the payload length in

@@ -64,6 +64,19 @@ class Transmission(C.Structure):
     _fields_ = [("shift_hz", C.c_int32), ("flush", C.c_int32), ("key", C.c_int32), ("power", C.c_float)]
 
 
+EV_START, EV_STOP, EV_LOST = 1, 2, 3
+
+
+class SignalEvent(C.Structure):
+    """b2s_signal_event: one change of the signal map (for EV_LOST, `key` events that did not fit the device log)."""
+
+    _fields_ = [("kind", C.c_int32), ("key", C.c_int32), ("shift_hz", C.c_int32), ("reserved", C.c_int32), ("frame", C.c_int64), ("time_ms", C.c_int64),
+                ("first_ms", C.c_int64), ("last_ms", C.c_int64)]
+
+    def astuple(self):
+        return (self.kind, self.key, self.shift_hz, self.frame, self.time_ms, self.first_ms, self.last_ms)
+
+
 class Result(C.Structure):
     _fields_ = [
         ("n_transmissions", C.c_int32),
@@ -204,6 +217,9 @@ def lib():
         L.b2s_band_get_spectrogram.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int)]
         L.b2s_band_get_transmissions.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
         L.b2s_band_get_signals.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
+        L.b2s_band_set_event_log.argtypes = [C.c_void_p, C.c_int]
+        for f in ("b2s_band_get_events", "b2s_host_transmission_get_events"):
+            getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int)]
         L.b2s_averager_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
         L.b2s_averager_destroy.argtypes = [C.c_void_p]
         L.b2s_averager_push.argtypes = [C.c_void_p, C.c_void_p]
@@ -239,6 +255,14 @@ def _check(rc: int):
 
 def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _get_events(fn, handle, cap: int, consume: bool):
+    """(the oldest `cap` events as (kind, key, shift_hz, frame, time_ms, first_ms, last_ms), the number that were queued)"""
+    ev = (SignalEvent * max(cap, 1))()
+    count = C.c_int()
+    _check(fn(handle, C.cast(ev, C.c_void_p), cap, 1 if consume else 0, C.byref(count)))
+    return [ev[i].astuple() for i in range(min(count.value, cap))], count.value
 
 
 class _Handle:
@@ -485,6 +509,17 @@ class Band(_Handle):
         k = min(count.value, cap)
         return keys[:k], first[:k], last[:k], power[:k]
 
+    def set_event_log(self, enable: bool = True):
+        """b2s_band_set_event_log: log every start and stop of a transmission in the pushes after this call."""
+        _check(lib().b2s_band_set_event_log(self._h, 1 if enable else 0))
+
+    def get_events(self, cap: int = 65536, consume: bool = True):
+        """The oldest `cap` signal events of the finished pushes: [(kind, key, shift_hz, frame, time_ms, first_ms, last_ms)]."""
+        return _get_events(lib().b2s_band_get_events, self._h, cap, consume)[0]
+
+    def event_count(self) -> int:
+        return _get_events(lib().b2s_band_get_events, self._h, 0, False)[1]
+
 
 # ---- host helpers (reference semantics) ----
 def get_fft(sample_rate_hz: int, max_step_hz: int) -> int:
@@ -521,6 +556,10 @@ class HostTransmission(_Handle):
 
     def reset(self):
         _check(lib().b2s_host_transmission_reset(self._h))
+
+    def get_events(self, cap: int = 65536, consume: bool = True):
+        """The tracker's signal event log (b2s_host_transmission_get_events), as Band.get_events returns it."""
+        return _get_events(lib().b2s_host_transmission_get_events, self._h, cap, consume)[0]
 
 
 def _pack(fn, time_ms: int, frequency_hz: int, sample_rate_hz: int, data: np.ndarray, count: int, header: int) -> bytes:

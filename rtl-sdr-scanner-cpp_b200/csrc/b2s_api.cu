@@ -50,6 +50,15 @@ int fail(int code, const char* fmt, ...) {
     if (err__ != cudaSuccess) return fail(B2S_E_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(err__), __FILE__, __LINE__); \
   } while (0)
 
+// copies up to `cap` of the queued events to `out`, reports how many there are and drops the copied ones when asked to
+template <class Queue>
+static void hand_out_events(Queue& q, b2s_signal_event* out, int cap, int consume, int* count) {
+  const int total = static_cast<int>(q.size()), n = out ? std::max(0, std::min(cap, total)) : 0;
+  std::copy(q.begin(), q.begin() + n, out);
+  *count = total;
+  if (consume) q.erase(q.begin(), q.begin() + n);
+}
+
 // The owners of the library's CUDA resources. Each frees what it holds when it is destroyed and can be moved but not copied, so an
 // object's resources go with the object and an early return frees what a function had allocated.
 
@@ -1214,6 +1223,30 @@ int b2s_band_get_signals(b2s_band* b, int32_t* keys, int64_t* first, int64_t* la
   return 0;
 }
 
+int b2s_band_set_event_log(b2s_band* b, int enable) {
+  if (!b) return fail(B2S_E_INVALID, "NULL band");
+  std::lock_guard<std::mutex> lock(b->mutex);
+  b->event_log = enable != 0;
+  if (!b->event_log) {  // the slots' record buffers go once no chunk in flight writes them
+    CU(cudaSetDevice(b->engine->device));
+    int rc = b->drain();
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(b->track_stream));
+    for (auto& s : b->slots) s.d_log = DevBuf<TrackEvent>();
+  }
+  return 0;
+}
+
+int b2s_band_get_events(b2s_band* b, b2s_signal_event* out, int cap, int consume, int* count) {
+  if (!b || !count) return fail(B2S_E_INVALID, "NULL argument");
+  std::lock_guard<std::mutex> lock(b->mutex);
+  int rc = b->drain();
+  if (rc) return rc;
+  std::lock_guard<std::mutex> lk(b->qmutex);
+  hand_out_events(b->events, out, cap, consume, count);
+  return 0;
+}
+
 // ---- stand-alone operators ----
 int b2s_averager_create(b2s_engine* e, int size, int group_size, b2s_averager** out) {
   if (!e || !out || size < 1 || group_size < 1) return fail(B2S_E_INVALID, "bad argument");
@@ -1577,6 +1610,8 @@ struct b2s_host_transmission : DeviceQueries {
   b2s_band_config cfg{};
   Tracker tracker;
   std::vector<float> history;  // the last Y rows of q before the current call, oldest -> newest (zeros before any data)
+  std::vector<b2s_signal_event> events;  // the tracker's signal event log
+  int64_t frames_pushed = 0;
   // current call
   const float* box = nullptr;
   const float* q = nullptr;
@@ -1646,7 +1681,13 @@ int b2s_host_transmission_create(const b2s_band_config* cfg, b2s_host_transmissi
   p.timeout = cfg->timeout_ms;
   p.max_time = cfg->max_time_ms;
   h->history.assign(static_cast<size_t>(cfg->grouping_y) * cfg->fft_size, 0.0f);  // Averager::reset fills the ring with zeros
+  h->tracker.log = &h->events;
   *out = h.release();
+  return 0;
+}
+int b2s_host_transmission_get_events(b2s_host_transmission* h, b2s_signal_event* out, int cap, int consume, int* count) {
+  if (!h || !count) return fail(B2S_E_INVALID, "NULL argument");
+  hand_out_events(h->events, out, cap, consume, count);
   return 0;
 }
 int b2s_host_transmission_destroy(b2s_host_transmission* h) {
@@ -1709,6 +1750,8 @@ int b2s_host_transmission_push(b2s_host_transmission* h, const float* box_rows, 
   }
   std::vector<Tracker::FrameState> states;
   const DetectEntry* ep = entries.empty() ? nullptr : entries.data();
+  h->tracker.log_frame_base = h->frames_pushed;
+  h->frames_pushed += T;
   const auto run_t0 = std::chrono::steady_clock::now();
   int rc = h->tracker.run(ep, begin.data(), static_cast<size_t>(T), t0_ms, frame_period_ms, 0, *h, tx_count != nullptr || tx != nullptr, watch, states);
   h->last_run_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - run_t0).count();

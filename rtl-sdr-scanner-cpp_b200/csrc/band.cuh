@@ -56,6 +56,9 @@ struct PushSlot {
   DevBuf<TrackResult> d_result;
   DevBuf<b2s_transmission> d_tx;  // [N] the push's whole sorted list (TrackArgs::tx)
   PinBuf<TrackResult> h_result;
+  DevBuf<TrackEvent> d_log;  // [N] the signal event records of the chunk's K4 (TrackArgs::log); allocated while the log is on
+  bool log_on = false;       // the event log was on when the chunk was enqueued
+  int64_t frame_base = 0;    // frames pushed to the band before the chunk's first
   Event sorted_done, tev[2];
   bool host_track = false;  // this chunk's bookkeeping runs on the host (the caller asked for every frame's list)
   int epoch = 0;            // reset_epoch when the chunk was enqueued
@@ -139,6 +142,10 @@ struct b2s_band : public DeviceQueries {
   std::vector<b2s_transmission> mailbox;  // the complete list, strongest first (guarded by qmutex against reset_buffers)
   int reset_epoch = 0;                    // bumped by reset_buffers
   int stat_entries = 0, stat_rows = 0;
+  // the signal event log (b2s_band_set_event_log): the events of the finished chunks, oldest first (guarded by qmutex)
+  bool event_log = false;
+  std::deque<b2s_signal_event> events;
+  int64_t frames_pushed = 0;  // frames enqueued since the band was created: b2s_signal_event::frame of the next chunk's first
 
   // profiling
   bool profiling = false;
@@ -659,6 +666,9 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
   int rc;
   s.epoch = reset_epoch;
   s.host_track = out && out->frame_tx_count;  // every frame's list is wanted: the bookkeeping runs on the host (tracker.h)
+  s.log_on = event_log;
+  s.frame_base = frames_pushed;
+  if (s.log_on && !s.host_track && (rc = s.d_log.alloc(n))) return rc;
   if (s.host_track && (rc = state_to_host_tracker())) return rc;
   s.dense_q_on = out && out->noise_sub_db;
   s.dense_avg_on = out && out->avg_db;
@@ -889,6 +899,8 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
     ta.tx = s.d_tx.p;
     ta.hit = d_track_hit.p;
     ta.sort_keys = d_track_sort.p;
+    ta.log = s.log_on ? s.d_log.p : nullptr;
+    ta.log_cap = n;
     // k_track runs the push unless it would pass its shared tables; then it leaves the map untouched and sets the result's
     // hand-off flag, and k_track_wide, always enqueued behind it, runs the push from the same map. Otherwise k_track_wide exits.
     const bool len14 = run_len_bits(cfg.fft_size) == 14;
@@ -938,6 +950,7 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
   sum_cur ^= 1;
   avg_frames = std::min(avg_frames + T, Y);
   ring_cur = ring_out;
+  frames_pushed += T;
   prof.frames += T;
   prof.spectral_launches += 1;
   prof.detect_launches += 1;  // k_detect (+ the two small list-ordering kernels, timed with it)
@@ -980,6 +993,15 @@ int b2s_band::finish_chunk(PushSlot& s) {
       std::lock_guard<std::mutex> lk(qmutex);
       if (s.epoch == reset_epoch) mailbox.swap(list);  // (a reset issued after this chunk was enqueued has emptied the mailbox: keep it so)
     }
+    if (s.log_on && r.n_log > 0) {  // the chunk's signal events: in-launch frames become frames of the band
+      std::vector<TrackEvent> rec(std::min(r.n_log, n));
+      CU(cudaMemcpyAsync(rec.data(), s.d_log.p, sizeof(TrackEvent) * rec.size(), cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      prof.d2h_bytes += sizeof(TrackEvent) * rec.size();
+      std::lock_guard<std::mutex> lk(qmutex);
+      for (const TrackEvent& e : rec) events.push_back(b2s_signal_event{e.kind, e.key, e.shift_hz, 0, s.frame_base + e.frame, e.time, e.first, e.last});
+      if (r.n_log > n) events.push_back(b2s_signal_event{B2S_EV_LOST, r.n_log - n, 0, 0, events.back().frame, events.back().time_ms, 0, 0});
+    }
     if (profiling && s.tev[0]) {
       float ms = 0.0f;
       CU(cudaEventElapsedTime(&ms, s.tev[0], s.tev[1]));
@@ -1009,8 +1031,16 @@ int b2s_band::finish_chunk(PushSlot& s) {
     std::vector<Tracker::FrameState> states;
     tracker.p.center = s.center;
     Tracker::Watch watch{s.n_watch, s.watch_key, s.h_watch_max.p, s.h_cand_flag.p};
+    std::vector<b2s_signal_event> logged;
+    tracker.log = s.log_on ? &logged : nullptr;
+    tracker.log_frame_base = s.frame_base;
     rc = tracker.run(s.h_entries.p, h_off, T, s.t0_ms, s.period_ms, s.frame_offset, *this, true, watch, states);
+    tracker.log = nullptr;
     if (rc) return rc;
+    if (!logged.empty()) {
+      std::lock_guard<std::mutex> lk(qmutex);
+      events.insert(events.end(), logged.begin(), logged.end());
+    }
     prof.tracker_host_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
     // the mailbox after the last frame of this chunk (Notification::notify, transmission.cpp:67)
     mailbox.clear();

@@ -19,6 +19,14 @@
 // m_power (only read when the list is emitted) is taken for the last frame of the push from K2's boxcar row of that frame.
 // Tie rules left open by the reference's unstable std::sort are the oracle's: candidates (power desc, bin asc), transmissions
 // (power desc, key asc).
+//
+// The signal event log (b2s_signal_event; TrackArgs::log, null = off): where an event frame inserts a key the kernels append a
+// START record, where clearSignals drops one a STOP record with the Signal's two times, in the order Transmission::process makes
+// the changes: a frame's inserts first, then its erasures in ascending key. k_track appends from thread 0, which alone edits its
+// map; k_track_wide from thread 0 at an insert, and in clearSignals from the thread that holds the erased key, at the key's rank
+// among the erased, which is its index minus its rank among the kept that the compaction scan computes. The number of records
+// is published in the epilogue with the rest of the result, so a k_track that hands off leaves no count behind: k_track_wide
+// counts from 0 and writes over what k_track had appended.
 #pragma once
 #include "../../include/b2s.h"
 #include "detect.cuh"
@@ -57,11 +65,18 @@ struct TrackMap {
   float* power;
 };
 
+struct TrackEvent {  // one record of the signal event log
+  int kind, key, shift_hz;  // B2S_EV_START / B2S_EV_STOP, the map key, b2s_transmission::shift_hz of the key
+  int frame;                // in-launch frame index
+  long long time, first, last;
+};
+
 struct TrackResult {  // what the host reads back per push
   int n_tx, n_entries, max_count;
   int handoff;  // k_track stopped before writing any state and left the push to k_track_wide (which keeps the flag set)
   long long last_now;
-  int n_evals, n_events, n_best, pad;  // work counters of the push: block evaluations, event frames replayed, getBestIndex calls
+  int n_evals, n_events, n_best;  // work counters of the push: block evaluations, event frames replayed, getBestIndex calls
+  int n_log;                      // records the push appended to TrackArgs::log, also past log_cap (written only when the log is on)
   b2s_transmission tx[B2S_MAX_TX];     // the first B2S_MAX_TX of TrackArgs::tx
 };
 
@@ -88,6 +103,8 @@ struct TrackArgs {
   b2s_transmission* tx;            // [N] getSortedTransmissions after the last frame
   unsigned int* hit;               // k_track_wide: [N][kTrackWords] the keys' hit words of a block
   unsigned long long* sort_keys;   // k_track_wide: [N rounded up to a power of two] sort scratch
+  TrackEvent* log;                 // [log_cap] the push's signal events in order, or null: no log. The count is TrackResult::n_log
+  int log_cap;
 };
 
 __device__ __forceinline__ long long track_frame_time(long long t0, double period, long long k) {
@@ -125,7 +142,11 @@ __device__ __forceinline__ bool track_within_margin(const int* keys, int n, int 
   const int i = track_lower_bound(keys, n, index - margin);
   return i < n && keys[i] <= index + margin;
 }
-__device__ __forceinline__ void track_write_header(const TrackArgs& a, int n_tx, long long last_now, int handoff, int n_evals, int n_events, int n_best) {
+// record `at` of the log; records past the capacity are counted, not stored
+__device__ __forceinline__ void track_log(const TrackArgs& a, int at, int kind, int key, int frame, long long now, long long first, long long last) {
+  if (at < a.log_cap) a.log[at] = TrackEvent{kind, key, track_tuned(track_index_to_shift(a.p, key), a.p.tuning_step), frame, now, first, last};
+}
+__device__ __forceinline__ void track_write_header(const TrackArgs& a, int n_tx, long long last_now, int handoff, int n_evals, int n_events, int n_best, int n_log) {
   TrackResult* r = a.result;
   r->n_tx = n_tx;
   r->n_entries = a.n_frames > 0 ? a.offsets[a.n_frames] : 0;
@@ -135,6 +156,7 @@ __device__ __forceinline__ void track_write_header(const TrackArgs& a, int n_tx,
   r->n_evals = n_evals;
   r->n_events = n_events;
   r->n_best = n_best;
+  if (a.log) r->n_log = n_log;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -150,6 +172,7 @@ struct TrackShared {
   long long time[kTrackFrames];                 // frame clock of the block's frames
   int votes[128], tied[128];                    // getBestIndex scratch (thread 0)
   int changed, handoff, best_key;
+  int n_log;                        // signal event records appended so far (thread 0)
   int row_idx[128];                 // getBestIndex: first maximum of each ring row (-1 = below the start level)
   // event-frame scratch (the output lists reuse it after the last frame)
   int n_cand, n_open;
@@ -240,6 +263,7 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track(const TrackArgs a) {
   // ---- load the map; a map larger than the shared tables is k_track_wide's ----
   if (tid == 0) {
     s.n = *a.state.n;
+    s.n_log = 0;
     s.handoff = s.n > kMaxSignals ? 1 : 0;
     if (s.handoff) a.result->handoff = 1;
   }
@@ -432,6 +456,7 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track(const TrackArgs a) {
                 s.last[pos] = ev_now;
                 s.n += 1;
                 s.changed = 1;
+                if (a.log) track_log(a, s.n_log++, B2S_EV_START, key, te, ev_now, ev_now, ev_now);
               }
             }
           }
@@ -460,6 +485,7 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track(const TrackArgs a) {
           for (int i = 0; i < s.n; ++i) {
             if (s.last[i] + p.timeout <= ev_now || s.first[i] + p.max_time <= ev_now) {
               s.changed = 1;
+              if (a.log) track_log(a, s.n_log++, B2S_EV_STOP, s.key[i], te, ev_now, s.first[i], s.last[i]);
               continue;
             }
             s.key[w] = s.key[i];
@@ -519,7 +545,7 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track(const TrackArgs a) {
   }
   if (tid == 0) {
     *a.state.n = K;
-    track_write_header(a, K, last_now, 0, n_evals, n_events, n_best);
+    track_write_header(a, K, last_now, 0, n_evals, n_events, n_best, s.n_log);
   }
 }
 
@@ -537,6 +563,7 @@ struct TrackWideShared {
   long long time[kTrackFrames];
   int votes[128], tied[128];                    // getBestIndex scratch (thread 0)
   int changed, best_key;
+  int n_log;                                    // signal event records appended so far
   int row_idx[128];
   int n_open;
   int warp_sum[kTrackThreads / 32];
@@ -636,7 +663,10 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track_wide(const TrackArgs
   const int gh = p.group_size / 2, margin = track_margin(p.group_size);
   int n_evals = 0, n_events = 0, n_best = 0;
 
-  if (tid == 0) s.n = *a.state.n;
+  if (tid == 0) {
+    s.n = *a.state.n;
+    s.n_log = 0;
+  }
   __syncthreads();
 
   for (int bs = 0; bs < T; bs += kTrackFrames) {  // k_track's block walk
@@ -799,6 +829,7 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track_wide(const TrackArgs
               last[pos] = ev_now;
               s.n = nk + 1;
               s.changed = 1;
+              if (a.log) track_log(a, s.n_log++, B2S_EV_START, bk, te, ev_now, ev_now, ev_now);
             }
           }
           __syncthreads();
@@ -816,9 +847,10 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track_wide(const TrackArgs
           if (h) last[i] = ev_now;
         }
         __syncthreads();
-        // clearSignals: a stable compaction in place, 1024 keys at a time (a kept key only moves down, past keys already read)
+        // clearSignals: a stable compaction in place, 1024 keys at a time (a kept key only moves down, past keys already read).
+        // Key i is the (i - at)-th erased one when `at` kept keys precede it: its place among the frame's STOP records.
         {
-          const int nk = s.n;
+          const int nk = s.n, log_base = s.n_log;
           int w = 0;
           for (int c = 0; c < nk; c += kTrackThreads) {
             const int i = c + tid;
@@ -837,6 +869,8 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track_wide(const TrackArgs
               key[at] = k;
               first[at] = f;
               last[at] = l;
+            } else if (a.log && i < nk) {
+              track_log(a, log_base + i - at, B2S_EV_STOP, k, te, ev_now, f, l);
             }
             w += total;
             __syncthreads();
@@ -844,6 +878,7 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track_wide(const TrackArgs
           if (tid == 0 && w != nk) {
             s.n = w;
             s.changed = 1;
+            s.n_log = log_base + nk - w;
           }
         }
         __syncthreads();
@@ -885,7 +920,7 @@ __global__ void __launch_bounds__(kTrackThreads, 1) k_track_wide(const TrackArgs
   }
   if (tid == 0) {
     *a.state.n = K;
-    track_write_header(a, K, last_now, 1, n_evals, n_events, n_best);
+    track_write_header(a, K, last_now, 1, n_evals, n_events, n_best, s.n_log);
   }
 }
 
