@@ -220,6 +220,24 @@ int b2s_band_set_event_log(b2s_band* b, int enable);
  * events copied out (and only those) are dropped from the log */
 int b2s_band_get_events(b2s_band* b, b2s_signal_event* out, int cap, int consume, int* count);
 
+/* ---- snapshots: save a band's whole state and restore it into another band, in this process or another, on any engine ----
+ * A band restored from a snapshot continues exactly like the band that saved it: the noise thresholds of every centre visited, the
+ * Averager, the live signals, the spectrogram accumulators, the frame counter of the event log, the current centre and range, the
+ * mailbox, the spectrogram rows and events not yet collected, the statistics since the last sync and the detection capacity.
+ * Profiling counters and the attachment to a recorder bank are not part of it (attach the restored bank again).
+ * The snapshot is an opaque, versioned, checksummed byte string in HOST memory; its format is internal (DESIGN.md §3) and a load of
+ * another format version is refused.
+ * b2s_band_save_state first finishes every outstanding push (as b2s_band_sync does, but it collects and resets nothing). Calling it
+ * with cap too small (including buf == NULL, cap == 0) returns B2S_E_INVALID with *written = the required size, as the b2s_pack_*
+ * functions do. */
+int b2s_band_save_state(b2s_band* b, void* buf, size_t cap, size_t* written);
+/* Replace the band's whole state with a saved one. The band may be new or used, on any engine or device, synchronous or asynchronous,
+ * host or device IQ. Outstanding pushes are finished first. The band must have been created with the snapshot's config, except for
+ * center_hz, range_lo_hz and range_hi_hz (taken from the snapshot), flags, max_frames_per_push and detect_capacity (the detection
+ * capacity becomes the larger of the band's and the snapshot's); floats and B2S_WINDOW_USER taps are compared bit for bit.
+ * A refused load (B2S_E_INVALID: damaged, truncated or incompatible snapshot; B2S_E_NOMEM) changes nothing else. */
+int b2s_band_load_state(b2s_band* b, const void* buf, size_t len);
+
 /* ---- stand-alone operators (operator-level parity with the reference's unit tests) ---- */
 /* device-backed Averager with the reference's surface (averager.h:8-28) */
 typedef struct b2s_averager b2s_averager;
@@ -348,6 +366,12 @@ int b2s_recorder_bank_push(b2s_recorder_bank* k, const void* iq, size_t n_sample
    with consume != 0 the chunks copied out (and only those) are dropped */
 int b2s_recorder_bank_flush(b2s_recorder_bank* k, int channel, int8_t* chunks /*[cap][chunk_samples][2]*/, int64_t* times_ms,
                             int cap, int consume, int* count, int* chunk_samples);
+/* Snapshot of a bank (conventions of b2s_band_save_state / b2s_band_load_state): the raw-sample carry and, per channel, whether it
+ * records, its rotator and stream position, its rows of every stage's carry and its unflushed chunks. Saving first settles the piece
+ * an asynchronous band left pending. A load needs the same sample rate, bandwidth, iq_format, iq_scale and channel count;
+ * max_samples_per_push and the flags may differ. */
+int b2s_recorder_bank_save_state(b2s_recorder_bank* k, void* buf, size_t cap, size_t* written);
+int b2s_recorder_bank_load_state(b2s_recorder_bank* k, const void* buf, size_t len);
 
 /* Record from the band's own pushes: every later b2s_band_push also runs `bank` over the pushed stream, reading the IQ the band
  * has already staged on the device (or the caller's device pointer). bank == NULL detaches. (SdrDevice connects its recorders to

@@ -218,6 +218,11 @@ def lib():
         L.b2s_band_get_transmissions.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
         L.b2s_band_get_signals.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
         L.b2s_band_set_event_log.argtypes = [C.c_void_p, C.c_int]
+        for f in ("b2s_band", "b2s_recorder_bank"):
+            getattr(L, f + "_save_state").argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+            getattr(L, f + "_save_state").restype = C.c_int
+            getattr(L, f + "_load_state").argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+            getattr(L, f + "_load_state").restype = C.c_int
         for f in ("b2s_band_get_events", "b2s_host_transmission_get_events"):
             getattr(L, f).argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int)]
         L.b2s_averager_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
@@ -255,6 +260,23 @@ def _check(rc: int):
 
 def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _save_state(fn, handle) -> bytes:
+    """A b2s_*_save_state snapshot: one call for the size (it returns B2S_E_INVALID with the size), one for the bytes."""
+    need = C.c_size_t(0)
+    rc = fn(handle, None, 0, C.byref(need))
+    if need.value == 0:
+        _check(rc)
+    buf = np.empty(need.value, np.uint8)
+    _check(fn(handle, _ptr(buf), buf.size, C.byref(need)))
+    return buf[: need.value].tobytes()
+
+
+def _load_state(fn, handle, data) -> None:
+    data = bytes(data)
+    buf = np.frombuffer(data or b"\0", np.uint8)
+    _check(fn(handle, _ptr(buf), len(data)))
 
 
 def _get_events(fn, handle, cap: int, consume: bool):
@@ -520,6 +542,14 @@ class Band(_Handle):
     def event_count(self) -> int:
         return _get_events(lib().b2s_band_get_events, self._h, 0, False)[1]
 
+    def save_state(self) -> bytes:
+        """b2s_band_save_state: the band's whole state as an opaque snapshot (outstanding pushes are finished first)."""
+        return _save_state(lib().b2s_band_save_state, self._h)
+
+    def load_state(self, data: bytes):
+        """b2s_band_load_state: replace the band's whole state with a snapshot of a band created with the same config."""
+        _load_state(lib().b2s_band_load_state, self._h, data)
+
 
 # ---- host helpers (reference semantics) ----
 def get_fft(sample_rate_hz: int, max_step_hz: int) -> int:
@@ -715,6 +745,14 @@ class RecorderBank(_Handle):
         times = np.empty(k, np.int64)
         _check(lib().b2s_recorder_bank_flush(self._h, channel, _ptr(chunks), _ptr(times), k, 1 if consume else 0, C.byref(count), C.byref(cs)))
         return [(int(times[i]), chunks[i]) for i in range(k)]
+
+    def save_state(self) -> bytes:
+        """b2s_recorder_bank_save_state: every channel's position, carries and unflushed chunks as an opaque snapshot."""
+        return _save_state(lib().b2s_recorder_bank_save_state, self._h)
+
+    def load_state(self, data: bytes):
+        """b2s_recorder_bank_load_state: replace the bank's state with a snapshot of a bank of the same rate, bandwidth, format and size."""
+        _load_state(lib().b2s_recorder_bank_load_state, self._h, data)
 
 
 class RecorderAction(C.Structure):
