@@ -372,6 +372,22 @@ int b2s_recorder_bank_flush(b2s_recorder_bank* k, int channel, int8_t* chunks /*
  * max_samples_per_push and the flags may differ. */
 int b2s_recorder_bank_save_state(b2s_recorder_bank* k, void* buf, size_t cap, size_t* written);
 int b2s_recorder_bank_load_state(b2s_recorder_bank* k, const void* buf, size_t len);
+/* History: a recording can start at a sample already pushed to the bank, such as the first frame of a transmission that the band
+ * reports only some frames later.
+ * Keep the newest `samples` samples of the bank's stream on the device (0, the default: keep none). Every later push of the bank,
+ * stand-alone or through an attached band, appends its samples. Positions count the samples pushed to the bank since the last
+ * set_history or b2s_recorder_bank_load_state, which both empty the history. The call finishes the bank's outstanding work first.
+ * A refused call (B2S_E_NOMEM) keeps the previous history. The history is not part of a snapshot. */
+int b2s_recorder_bank_set_history(b2s_recorder_bank* k, size_t samples);
+/* The positions the history holds: [*oldest, *end). */
+int b2s_recorder_bank_history(b2s_recorder_bank* k, int64_t* oldest, int64_t* end);
+/* Recorder::startRecording, but from stream position `position` (oldest <= position <= end) instead of from the next push. The samples
+ * [position, end) are recorded at once ("catch-up"), cut every max_samples_per_push samples from `position`. The channel then continues
+ * with the following pushes. Its chunks are stamped from start_ms. Its bytes and chunk times equal those of a channel of a fresh
+ * stand-alone bank with the same settings, started with shift_hz and pushed [position, end) in those cuts (the first push at start_ms),
+ * then the same later pushes; for position == end that is b2s_recorder_bank_start. B2S_E_STATE when the channel records; B2S_E_INVALID
+ * for a position outside the history, or when the bank keeps none. */
+int b2s_recorder_bank_start_from(b2s_recorder_bank* k, int channel, int32_t shift_hz, int64_t position, int64_t start_ms);
 
 /* Record from the band's own pushes: every later b2s_band_push also runs `bank` over the pushed stream, reading the IQ the band
  * has already staged on the device (or the caller's device pointer). bank == NULL detaches. (SdrDevice connects its recorders to
@@ -399,6 +415,17 @@ int b2s_recorder_bank_load_state(b2s_recorder_bank* k, const void* buf, size_t l
  *     of the following samples continues the same recordings byte for byte. b2s_band_reset, b2s_band_set_center and noise learning do
  *     not touch the bank. */
 int b2s_band_attach_recorder_bank(b2s_band* b, b2s_recorder_bank* bank);
+/* Start channel `channel` of the band's attached bank at the first sample of band frame `frame` (counted like b2s_signal_event.frame),
+ * stamped with that frame's injected clock: b2s_recorder_bank_start_from at the frame's position. Refused (B2S_E_INVALID, nothing
+ * changes) when
+ * - no bank is attached or it keeps no history;
+ * - the frame is not yet pushed or no longer in the history;
+ * - the frame was pushed before the bank was attached, before its last set_history, before the band's last b2s_band_load_state,
+ *   or before the last b2s_band_set_center that changed the centre (that IQ belongs to another centre).
+ * b2s_band_reset does not limit it. B2S_E_STATE when the channel records. With B2S_FLAG_ASYNC the frame may lie in a push whose
+ * kernels are still running: the catch-up follows the bank's reads of it. Typical use: on B2S_REC_START from the scan policy, take
+ * the START event with the same shift_hz and call this with event.frame minus a pre-roll instead of b2s_recorder_bank_start. */
+int b2s_band_record_from(b2s_band* b, int channel, int32_t shift_hz, int64_t frame);
 
 #ifdef __cplusplus
 }

@@ -218,6 +218,12 @@ def lib():
         L.b2s_band_get_transmissions.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
         L.b2s_band_get_signals.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
         L.b2s_band_set_event_log.argtypes = [C.c_void_p, C.c_int]
+        L.b2s_recorder_bank_set_history.argtypes = [C.c_void_p, C.c_size_t]
+        L.b2s_recorder_bank_history.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.b2s_recorder_bank_start_from.argtypes = [C.c_void_p, C.c_int, C.c_int32, C.c_int64, C.c_int64]
+        L.b2s_band_record_from.argtypes = [C.c_void_p, C.c_int, C.c_int32, C.c_int64]
+        for f in ("b2s_recorder_bank_set_history", "b2s_recorder_bank_history", "b2s_recorder_bank_start_from", "b2s_band_record_from"):
+            getattr(L, f).restype = C.c_int
         for f in ("b2s_band", "b2s_recorder_bank"):
             getattr(L, f + "_save_state").argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
             getattr(L, f + "_save_state").restype = C.c_int
@@ -542,6 +548,11 @@ class Band(_Handle):
     def event_count(self) -> int:
         return _get_events(lib().b2s_band_get_events, self._h, 0, False)[1]
 
+    def record_from(self, channel: int, shift_hz: int, frame: int):
+        """b2s_band_record_from: start `channel` of the attached bank at band frame `frame` (as in the signal events), from the bank's
+        history, its chunks stamped with that frame's clock."""
+        _check(lib().b2s_band_record_from(self._h, channel, shift_hz, frame))
+
     def save_state(self) -> bytes:
         """b2s_band_save_state: the band's whole state as an opaque snapshot (outstanding pushes are finished first)."""
         return _save_state(lib().b2s_band_save_state, self._h)
@@ -745,6 +756,21 @@ class RecorderBank(_Handle):
         times = np.empty(k, np.int64)
         _check(lib().b2s_recorder_bank_flush(self._h, channel, _ptr(chunks), _ptr(times), k, 1 if consume else 0, C.byref(count), C.byref(cs)))
         return [(int(times[i]), chunks[i]) for i in range(k)]
+
+    def set_history(self, samples: int):
+        """b2s_recorder_bank_set_history: keep the newest `samples` samples of the stream on the device (0: none); empties the history."""
+        _check(lib().b2s_recorder_bank_set_history(self._h, samples))
+
+    def history(self):
+        """(oldest, end): the stream positions the history holds, counted since the last set_history or load_state."""
+        oldest, end = C.c_int64(), C.c_int64()
+        _check(lib().b2s_recorder_bank_history(self._h, C.byref(oldest), C.byref(end)))
+        return oldest.value, end.value
+
+    def start_from(self, channel: int, shift_hz: int, position: int, start_ms: int):
+        """b2s_recorder_bank_start_from: start `channel` at stream position `position` of the history; [position, end) is recorded
+        at once, its chunks stamped from start_ms."""
+        _check(lib().b2s_recorder_bank_start_from(self._h, channel, shift_hz, position, int(start_ms)))
 
     def save_state(self) -> bytes:
         """b2s_recorder_bank_save_state: every channel's position, carries and unflushed chunks as an opaque snapshot."""

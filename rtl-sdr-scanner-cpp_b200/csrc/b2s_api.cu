@@ -673,6 +673,15 @@ struct b2s_recorder_bank {
     }
   };
   std::vector<Channel> ch;
+  // History (b2s_recorder_bank_set_history): the newest hist_cap raw samples of the stream, stream position p in ring slot
+  // p % hist_cap. hist_end counts the samples pushed since the last set_history or load; hist_epoch changes whenever the history is
+  // emptied, so that positions taken before are recognised as void. gather holds a catch-up piece whose samples (with the hc before
+  // it) wrap around the ring's end.
+  DevBuf<unsigned char> hist, gather;
+  size_t hist_cap = 0;
+  long long hist_end = 0;
+  uint64_t hist_epoch = 0;
+  long long hist_oldest() const { return hist_end - std::min<long long>(hist_end, static_cast<long long>(hist_cap)); }
   size_t raw_bytes() const { return iq_format == B2S_IQ_CS8 ? 2 : 8; }
 };
 
@@ -756,13 +765,14 @@ int bank_create(b2s_engine* e, int32_t sample_rate_hz, int32_t bandwidth_hz, int
   return 0;
 }
 
-// What a push of n_samples does: the recording channels (p.rec), each one's geometry in every stage ([channel][stage], the return value)
-// and output count (p.produced, p.most). Reads the channels' stream positions and changes nothing.
-std::vector<StageChan> bank_plan(const b2s_recorder_bank* k, size_t n_samples, b2s_recorder_bank::Launched& p) {
+// What a push of n_samples does: the recording channels (p.rec; only channel `only` when it is >= 0), each one's geometry in every
+// stage ([channel][stage], the return value) and output count (p.produced, p.most). Reads the channels' stream positions and changes
+// nothing.
+std::vector<StageChan> bank_plan(const b2s_recorder_bank* k, size_t n_samples, b2s_recorder_bank::Launched& p, int only = -1) {
   const int n_st = static_cast<int>(k->stages.size());
   p.rec.clear();
   for (int i = 0; i < k->n_ch; ++i)
-    if (k->ch[i].recording) p.rec.push_back(i);
+    if (k->ch[i].recording && (only < 0 || i == only)) p.rec.push_back(i);
   std::vector<StageChan> geo(p.rec.size() * n_st);
   p.produced.assign(p.rec.size(), 0);
   p.most = 0;
@@ -787,21 +797,32 @@ std::vector<StageChan> bank_plan(const b2s_recorder_bank* k, size_t n_samples, b
   return geo;
 }
 
+// the history ring's slot of stream position pos (pos < 0 is the carry of a catch-up's first piece, which no kernel reads)
+size_t hist_slot(const b2s_recorder_bank* k, long long pos) {
+  const long long cap = static_cast<long long>(k->hist_cap);
+  return static_cast<size_t>((pos % cap + cap) % cap);
+}
+
 // The device half of a push whose n_samples input samples are on the device at `in`: one launch per stage (per kLaunchChannels
 // channels), the carries, and (p.fetch) the copy of the channels' int8 outputs into h_out[p.slot], all on the bank's stream. Advances the
-// channels' stream positions. stage0_done (optional) is recorded once stage 0 and the raw carry no longer read `in`.
-int bank_launch(b2s_recorder_bank* k, const void* in, size_t n_samples, int64_t t0_ms, const std::vector<StageChan>& geo, const b2s_recorder_bank::Launched& p,
-                cudaEvent_t stage0_done) {
+// channels' stream positions.
+// raw_carry == nullptr: the stream's next samples. Stage 0 reads the shared raw carry and moves it on, and the samples are appended to
+// the history; stage0_done (optional) is recorded once none of this reads `in` any more.
+// Otherwise a catch-up piece (bank_start_from) whose stage 0 finds the hc samples before `in` at raw_carry; the shared raw carry and
+// the history stay as they are.
+int bank_launch(b2s_recorder_bank* k, const void* in, const void* raw_carry, size_t n_samples, int64_t t0_ms, const std::vector<StageChan>& geo,
+                const b2s_recorder_bank::Launched& p, cudaEvent_t stage0_done) {
   const int n_st = static_cast<int>(k->stages.size());
   const std::vector<int>& rec = p.rec;
   const int raw_kind = k->iq_format == B2S_IQ_CS8 ? 0 : 1;
+  const bool stream_push = raw_carry == nullptr;
   for (int si = 0; si < n_st; ++si) {
     auto& st = k->stages[si];
     const bool last = si + 1 == n_st;
     for (size_t c0 = 0; c0 < rec.size(); c0 += kLaunchChannels) {
       ResampleArgs a{};
       a.in = si == 0 ? in : static_cast<const void*>(st.buf.p + st.hc);
-      a.carry = si == 0 ? static_cast<const void*>(k->carry_raw.p) : static_cast<const void*>(st.buf.p);
+      a.carry = si > 0 ? static_cast<const void*>(st.buf.p) : stream_push ? static_cast<const void*>(k->carry_raw.p) : raw_carry;
       a.in_stride = si == 0 ? 0 : static_cast<long long>(st.stride);
       a.kind = si == 0 ? raw_kind : 2;
       a.iq_scale = k->iq_scale;
@@ -837,10 +858,21 @@ int bank_launch(b2s_recorder_bank* k, const void* in, size_t n_samples, int64_t 
         CU(cudaGetLastError());
       }
     }
-    if (si == 0) {  // the raw stream's carry, shared by every channel, moves with every push
+    if (si == 0 && stream_push) {  // the raw stream's carry, shared by every channel, moves with every push
       if (raw_kind == 0) k_shift_carry<short><<<1, 1024, st.hc * 2, k->stream>>>(static_cast<short*>(static_cast<void*>(k->carry_raw.p)), static_cast<const short*>(in), st.hc, n_samples);
       else k_shift_carry<double><<<1, 1024, st.hc * 8, k->stream>>>(static_cast<double*>(static_cast<void*>(k->carry_raw.p)), static_cast<const double*>(in), st.hc, n_samples);
       CU(cudaGetLastError());
+      if (k->hist_cap) {  // the push's newest hist_cap samples into the history ring, cut where the ring ends
+        const size_t bps = k->raw_bytes(), keep = std::min(n_samples, k->hist_cap);
+        const long long from = k->hist_end + static_cast<long long>(n_samples - keep);
+        const unsigned char* src = static_cast<const unsigned char*>(in) + (n_samples - keep) * bps;
+        for (size_t done = 0; done < keep;) {
+          const size_t at = hist_slot(k, from + static_cast<long long>(done)), m = std::min(keep - done, k->hist_cap - at);
+          CU(cudaMemcpyAsync(k->hist.p + at * bps, src + done * bps, m * bps, cudaMemcpyDeviceToDevice, k->stream));
+          done += m;
+        }
+      }
+      k->hist_end += static_cast<long long>(n_samples);
       if (stage0_done) CU(cudaEventRecord(stage0_done, k->stream));
     }
   }
@@ -903,7 +935,7 @@ int bank_push(b2s_recorder_bank* k, const void* iq, size_t n_samples, int64_t t0
     in = k->staging.p;
   }
   p.fetch = p.most > 0 && (out_iq || k->keep_chunks);
-  if ((rc = bank_launch(k, in, n_samples, t0_ms, geo, p, nullptr))) return rc;
+  if ((rc = bank_launch(k, in, nullptr, n_samples, t0_ms, geo, p, nullptr))) return rc;
   CU(cudaStreamSynchronize(k->stream));
   bank_take(k, p, out_iq, cap_samples, n_out);
   return 0;
@@ -922,12 +954,48 @@ int bank_feed(b2s_recorder_bank* k, const void* in, size_t n_samples, int64_t t0
   p.slot = k->has_pending ? k->pending.slot ^ 1 : 0;
   p.fetch = p.most > 0;
   CU(cudaStreamWaitEvent(k->stream, ready, 0));
-  rc = bank_launch(k, in, n_samples, t0_ms, geo, p, stage0_done);
+  rc = bank_launch(k, in, nullptr, n_samples, t0_ms, geo, p, stage0_done);
   if (rc) return rc;
   CU(cudaEventRecord(k->out_ready[p.slot], k->stream));
   if ((rc = bank_settle(k))) return rc;
   k->pending = std::move(p);
   k->has_pending = true;
+  return 0;
+}
+
+// Start `channel` at stream position `position` of the history (b2s_recorder_bank_start_from): the samples [position, end) run through
+// the channel alone at once, cut every max_in samples from `position` as a fresh bank's pushes would be, with seen counting from
+// `position`. Stage 0 reads each piece in the ring, with the hc samples before it as its carry (the first piece reads none: they
+// precede the channel's start); a piece whose span [start - hc, end) wraps around the ring's end is gathered first. Synchronous on
+// the bank's stream, which also orders it after every piece a band has fed.
+int bank_start_from(b2s_recorder_bank* k, int channel, int32_t shift_hz, long long position, int64_t start_ms, const char* who) {
+  int rc = bank_settle(k);
+  if (rc) return rc;
+  if (k->ch[channel].recording) return fail(B2S_E_STATE, "%s: channel %d is already recording", who, channel);
+  if (!k->hist_cap || position < k->hist_oldest() || position > k->hist_end)
+    return fail(B2S_E_INVALID, "%s: position %lld is outside the history [%lld, %lld)", who, position, k->hist_oldest(), k->hist_end);
+  CU(cudaSetDevice(k->engine->device));
+  start_channel(k->ch[channel], rotator_phase_inc(shift_hz, k->sample_rate));
+  const size_t bps = k->raw_bytes(), hc = static_cast<size_t>(k->stages[0].hc);
+  for (long long s = position; s < k->hist_end; s += static_cast<long long>(k->max_in)) {
+    const size_t n = static_cast<size_t>(std::min<long long>(static_cast<long long>(k->max_in), k->hist_end - s));
+    const size_t at = hist_slot(k, s);
+    const unsigned char* in = k->hist.p + at * bps;
+    if (at < hc || at + n > k->hist_cap) {
+      for (size_t done = 0; done < hc + n;) {
+        const size_t from = hist_slot(k, s - static_cast<long long>(hc - done)), m = std::min(hc + n - done, k->hist_cap - from);
+        CU(cudaMemcpyAsync(k->gather.p + done * bps, k->hist.p + from * bps, m * bps, cudaMemcpyDeviceToDevice, k->stream));
+        done += m;
+      }
+      in = k->gather.p + hc * bps;
+    }
+    b2s_recorder_bank::Launched p;
+    const std::vector<StageChan> geo = bank_plan(k, n, p, channel);
+    p.fetch = p.most > 0;
+    if ((rc = bank_launch(k, in, in - hc * bps, n, start_ms, geo, p, nullptr))) return rc;
+    CU(cudaStreamSynchronize(k->stream));
+    bank_take(k, p, nullptr, 0, nullptr);
+  }
   return 0;
 }
 
@@ -942,6 +1010,24 @@ int band_detach(b2s_band* b) {
   b->bank = nullptr;
   b->d_whole = DevBuf<unsigned char>();
   return rc ? rc : rc2;
+}
+
+// bank_feed of the piece of a band push that starts at frame `first` of the push, band frame `frame`, `frames` frames long. While the
+// bank keeps history the band notes where the piece sits in the bank's stream, for b2s_band_record_from.
+int band_feed(b2s_band* b, const void* in, int64_t frame, size_t first, size_t frames, int64_t t0_ms, double period_ms, cudaEvent_t ready,
+              cudaEvent_t stage0_done) {
+  b2s_recorder_bank* k = b->bank;
+  const long long position = k->hist_end;
+  const int rc = bank_feed(k, in, frames * static_cast<size_t>(b->cfg.frame_stride_samples), host::frame_time(t0_ms, period_ms, first), ready, stage0_done);
+  if (rc || !k->hist_cap) return rc;
+  if (b->hist_epoch != k->hist_epoch) {
+    b->hist_pieces.clear();
+    b->hist_epoch = k->hist_epoch;
+  }
+  b->hist_pieces.push_back({frame, static_cast<int64_t>(frames), position, t0_ms, period_ms, first});
+  const long long stride = b->cfg.frame_stride_samples;
+  while (!b->hist_pieces.empty() && b->hist_pieces.front().position + b->hist_pieces.front().n_frames * stride <= k->hist_oldest()) b->hist_pieces.pop_front();
+  return 0;
 }
 
 // ---- recorder bank snapshot: the raw-sample carry, then per channel its position, its rows of the stages' carries and its chunks ----
@@ -1051,6 +1137,8 @@ int bank_load(b2s_recorder_bank* k, const void* buf, size_t len) {
   }
   CU(cudaStreamSynchronize(k->stream));
   k->ch.swap(s_ch);
+  k->hist_end = 0;  // the history, which a snapshot does not hold, is of another stream
+  ++k->hist_epoch;
   return 0;
 }
 
@@ -1201,6 +1289,7 @@ int b2s_band_attach_recorder_bank(b2s_band* b, b2s_recorder_bank* k) {
   b->d_whole = std::move(whole);
   b->bank = k;
   k->band = b;
+  b->hist_pieces.clear();  // frames pushed before the attachment are not in the bank's history
   return 0;
 }
 int b2s_band_set_stream(b2s_band* b, void* cuda_stream) {
@@ -1231,9 +1320,9 @@ int b2s_band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, d
   const size_t bytes_per_sample = b->cfg.iq_format == B2S_IQ_CS8 ? 2 : 8;
   const size_t stride_bytes = static_cast<size_t>(b->cfg.frame_stride_samples) * bytes_per_sample;
   const bool on_device = (b->cfg.flags & B2S_FLAG_IQ_ON_DEVICE) != 0;
+  const int64_t frame0 = b->frames_pushed;  // the band frame of the push's first frame
   // An attached bank reads the push as pieces of up to max_frames frames (frame_stride_samples each), piece j stamped like frame
   // j * max_frames. A synchronous band settles each piece before it moves on; an asynchronous one leaves the newest piece pending.
-  const size_t stride = static_cast<size_t>(b->cfg.frame_stride_samples);
   auto settle_if_sync = [&]() { return b->bank && !b->async_mode ? bank_settle(b->bank) : 0; };
   if (b->bank && n_frames == 0) {
     const int rc = bank_settle(b->bank);
@@ -1245,7 +1334,7 @@ int b2s_band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, d
     for (size_t done = 0; done < n_frames && !rc;) {
       const size_t chunk = std::min(n_frames - done, static_cast<size_t>(b->max_frames));
       const char* piece = static_cast<const char*>(iq) + done * stride_bytes;
-      rc = b->bank ? bank_feed(b->bank, piece, chunk * stride, host::frame_time(t0_ms, frame_period_ms, done), b->push_ready, b->bank_read) : 0;
+      rc = b->bank ? band_feed(b, piece, frame0 + done, done, chunk, t0_ms, frame_period_ms, b->push_ready, b->bank_read) : 0;
       if (!rc) rc = b->push_chunk(piece, chunk, t0_ms, frame_period_ms, done, out);
       if (!rc) rc = settle_if_sync();
       done += chunk;
@@ -1279,7 +1368,7 @@ int b2s_band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, d
         CU(cudaEventRecord(b->copy_done[slot], b->copy_stream));
         b->prof.h2d_bytes += bytes;
         if (off + part < piece) return 0;
-        return bank_feed(b->bank, whole, piece * stride, host::frame_time(t0_ms, frame_period_ms, p0), b->copy_done[slot], b->bank_read);
+        return band_feed(b, whole, frame0 + p0, p0, piece, t0_ms, frame_period_ms, b->copy_done[slot], b->bank_read);
       };
       // d_whole is overwritten only after the bank has read the previous piece (still pending if the push that fed it failed)
       CU(cudaStreamWaitEvent(b->copy_stream, b->bank_read, 0));
@@ -1322,7 +1411,7 @@ int b2s_band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, d
       if (rc) return rc;
       CU(cudaStreamWaitEvent(b->stream, b->copy_done[slot], 0));
       // a chunk is a whole piece here (pipe = max_frames when the push is longer)
-      if (b->bank && (rc = bank_feed(b->bank, b->d_iq[slot].p, chunk * stride, host::frame_time(t0_ms, frame_period_ms, done), b->copy_done[slot], b->bank_prev_use[slot])))
+      if (b->bank && (rc = band_feed(b, b->d_iq[slot].p, frame0 + done, done, chunk, t0_ms, frame_period_ms, b->copy_done[slot], b->bank_prev_use[slot])))
         return rc;
       rc = b->push_chunk(b->d_iq[slot].p, chunk, t0_ms, frame_period_ms, done, nullptr);
       if (rc) return rc;
@@ -1404,6 +1493,7 @@ int b2s_band_set_center(b2s_band* b, int32_t center_hz, int32_t lo, int32_t hi) 
   std::lock_guard<std::mutex> lock(b->mutex);
   int rc = b->drain();
   if (rc) return rc;
+  if (center_hz != b->center) b->hist_pieces.clear();  // the history's IQ belongs to the old centre
   b->center = center_hz;
   b->tracker.p.center = center_hz;
   b->tracker.p.range_lo = lo;
@@ -1508,7 +1598,27 @@ int b2s_band_load_state(b2s_band* b, const void* buf, size_t len) {
   if (!b || !buf) return fail(B2S_E_INVALID, "b2s_band_load_state: NULL argument");
   std::lock_guard<std::mutex> lock(b->mutex);
   CU(cudaSetDevice(b->engine->device));
-  return b->load_state(buf, len);
+  const int rc = b->load_state(buf, len);
+  if (!rc) b->hist_pieces.clear();  // the frames pushed before belong to another stream
+  return rc;
+}
+
+int b2s_band_record_from(b2s_band* b, int channel, int32_t shift_hz, int64_t frame) {
+  const char* who = "b2s_band_record_from";
+  if (!b) return fail(B2S_E_INVALID, "%s: NULL band", who);
+  std::lock_guard<std::mutex> lock(b->mutex);
+  b2s_recorder_bank* k = b->bank;
+  if (!k || !k->hist_cap) return fail(B2S_E_INVALID, "%s: the band has no recorder bank that keeps history", who);
+  if (channel < 0 || channel >= k->n_ch) return fail(B2S_E_INVALID, "%s: bad channel", who);
+  const b2s_band::HistPiece* piece = nullptr;  // the newest piece that starts at or before `frame`
+  if (b->hist_epoch == k->hist_epoch) {
+    for (auto it = b->hist_pieces.rbegin(); it != b->hist_pieces.rend() && !piece; ++it)
+      if (it->frame <= frame) piece = &*it;
+  }
+  const long long position = piece ? piece->position + (frame - piece->frame) * static_cast<long long>(b->cfg.frame_stride_samples) : 0;
+  if (!piece || frame >= piece->frame + piece->n_frames || position < k->hist_oldest())
+    return fail(B2S_E_INVALID, "%s: frame %lld is not in the recorder bank's history", who, static_cast<long long>(frame));
+  return bank_start_from(k, channel, shift_hz, position, host::frame_time(piece->t0_ms, piece->period_ms, piece->first + static_cast<size_t>(frame - piece->frame)), who);
 }
 
 int b2s_band_set_event_log(b2s_band* b, int enable) {
@@ -1849,6 +1959,37 @@ int b2s_recorder_bank_save_state(b2s_recorder_bank* k, void* buf, size_t cap, si
 int b2s_recorder_bank_load_state(b2s_recorder_bank* k, const void* buf, size_t len) {
   if (!k || !buf) return fail(B2S_E_INVALID, "b2s_recorder_bank_load_state: NULL argument");
   return bank_load(k, buf, len);
+}
+
+int b2s_recorder_bank_set_history(b2s_recorder_bank* k, size_t samples) {
+  if (!k) return fail(B2S_E_INVALID, "b2s_recorder_bank_set_history: NULL bank");
+  int rc = bank_settle(k);
+  if (rc) return rc;
+  CU(cudaSetDevice(k->engine->device));
+  CU(cudaStreamSynchronize(k->stream));
+  const size_t bps = k->raw_bytes(), hc = static_cast<size_t>(k->stages[0].hc);
+  if (samples > (SIZE_MAX / bps) - k->max_in - hc) return fail(B2S_E_NOMEM, "b2s_recorder_bank_set_history: %zu samples do not fit in memory", samples);
+  DevBuf<unsigned char> ring, gather;  // allocated before anything changes: a refusal keeps the previous history
+  if (samples && ((rc = ring.alloc(samples * bps)) || (rc = gather.alloc((k->max_in + hc) * bps)))) {
+    cudaGetLastError();  // the failed allocation is not an error of later calls
+    return rc;
+  }
+  k->hist = std::move(ring);
+  k->gather = std::move(gather);
+  k->hist_cap = samples;
+  k->hist_end = 0;
+  ++k->hist_epoch;
+  return 0;
+}
+int b2s_recorder_bank_history(b2s_recorder_bank* k, int64_t* oldest, int64_t* end) {
+  if (!k || !oldest || !end) return fail(B2S_E_INVALID, "b2s_recorder_bank_history: NULL argument");
+  *oldest = k->hist_oldest();
+  *end = k->hist_end;
+  return 0;
+}
+int b2s_recorder_bank_start_from(b2s_recorder_bank* k, int channel, int32_t shift_hz, int64_t position, int64_t start_ms) {
+  if (!k || channel < 0 || channel >= k->n_ch) return fail(B2S_E_INVALID, "b2s_recorder_bank_start_from: bad channel");
+  return bank_start_from(k, channel, shift_hz, position, start_ms, "b2s_recorder_bank_start_from");
 }
 
 // self-test of the exact constant division (k_check_div_const above)

@@ -113,6 +113,19 @@ struct b2s_band : public DeviceQueries {
   b2s_recorder_bank* bank = nullptr;
   DevBuf<unsigned char> d_whole;
   Event bank_prev_use[2], push_ready, bank_read;
+  // The pieces fed to the bank while it keeps history, oldest first (b2s_band_record_from): the band frame and bank stream position of
+  // each piece's first frame, and the clock of its push (frame `first` of the push starts the piece). Pieces that left the history
+  // are dropped. Emptied when a bank is attached, when the centre changes and by a load; rows of an earlier history of the bank
+  // (another hist_epoch) are void.
+  struct HistPiece {
+    int64_t frame, n_frames;
+    long long position;
+    int64_t t0_ms;
+    double period_ms;
+    size_t first;
+  };
+  std::deque<HistPiece> hist_pieces;
+  uint64_t hist_epoch = 0;
   int max_frames = 0;
   int slot_capacity = 0;  // detection entries per frame
   int detect_bins = kDetectBinsPerCta;  // bins per K2 CTA (DetectArgs::bins_per_cta)
