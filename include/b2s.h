@@ -427,6 +427,44 @@ int b2s_band_attach_recorder_bank(b2s_band* b, b2s_recorder_bank* bank);
  * the START event with the same shift_hz and call this with event.frame minus a pre-roll instead of b2s_recorder_bank_start. */
 int b2s_band_record_from(b2s_band* b, int channel, int32_t shift_hz, int64_t frame);
 
+/* ---- auto-record: the band drives its attached bank the way SdrDevice::updateRecordings drives m_recorders (sdr_device.cpp:82-144) ----
+ * After each push with at least one frame is finished, the band runs the reference's recorder assignment on that push's mailbox (the
+ * list b2s_band_sync would return) at the clock of the push's last frame, and starts and stops the bank's channels itself. With a
+ * synchronous band that happens before b2s_band_push returns; with B2S_FLAG_ASYNC in the next b2s_band_push (before it feeds the bank)
+ * or b2s_band_sync, whichever comes first, after the push's bookkeeping has finished. The actions are exactly those a b2s_scan_policy
+ * with n_channels recorders returns from b2s_scan_policy_notify for the same lists (its recorder half: hopping stays the caller's).
+ *   - START: the band takes the latest START of the entry's key that K4 (or the host tracker) logged, and starts the channel at
+ *     max(START frame - preroll_frames, the oldest frame b2s_band_record_from accepts), stamped with that frame's clock: what
+ *     b2s_band_record_from does at that frame. All channels started by one decision catch up together. It starts the channel like
+ *     b2s_recorder_bank_start instead (from the next push on, from_frame = -1) when the bank keeps no history, when
+ *     b2s_band_record_from would refuse the START frame, when the START was logged before auto-record was enabled, or when the device
+ *     log lost records (B2S_EV_LOST) at or after it. preroll_frames = 0 without history is exactly the reference's behaviour.
+ *   - STOP stops the channel as b2s_recorder_bank_stop does (Recorder::stopRecording drops what was not flushed). FLUSH and NONE_FREE
+ *     only report: collecting chunks with b2s_recorder_bank_flush stays the caller's.
+ *   - The START records come from an internal log that does not depend on b2s_band_set_event_log: with the event log off,
+ *     b2s_band_get_events still returns nothing, and consuming events does not affect auto-record. The band's own results (mailbox,
+ *     map, spectrogram rows, events) are bit for bit those of the same band without auto-record.
+ * Enabling needs an attached bank whose channels are all idle (B2S_E_INVALID without a bank, B2S_E_STATE with a recording channel;
+ * nothing changes). While it is on, b2s_recorder_bank_start, b2s_recorder_bank_stop, b2s_recorder_bank_start_from and
+ * b2s_band_record_from on the bank return B2S_E_STATE and change nothing. Enabling it again while on only changes preroll_frames.
+ * Turning it off (enable = 0, detaching the bank, destroying either object, b2s_band_load_state) leaves the channels as they are, for
+ * the caller to drive, and drops a decision not yet made. b2s_band_reset and b2s_band_set_center stop no recording: the next mailbox
+ * does, as in the reference. Auto-record is not part of a snapshot. */
+int b2s_band_set_auto_record(b2s_band* b, int enable, int32_t preroll_frames);
+typedef struct b2s_auto_record_action {
+  int32_t kind;        /* B2S_REC_START / STOP / FLUSH / NONE_FREE, as b2s_recorder_action */
+  int32_t channel;     /* bank channel, -1 for NONE_FREE */
+  int32_t shift_hz;
+  int32_t key;         /* map key of the transmission */
+  int64_t frame;       /* band frame of the push's last frame: when the reference would have acted */
+  int64_t from_frame;  /* START: the band frame the recording starts at; -1 = started at the next push (no usable history) */
+  int64_t time_ms;     /* injected clock of `frame`; START: the clock of from_frame, which stamps the chunks */
+  int64_t duration_ms; /* STOP: Recorder::getDuration() */
+} b2s_auto_record_action;
+/* the actions taken, oldest first (conventions of b2s_band_get_events): up to `cap` are copied, *count is the number available; with
+ * consume != 0 the actions copied out (and only those) are dropped */
+int b2s_band_get_auto_record_actions(b2s_band* b, b2s_auto_record_action* out, int cap, int consume, int* count);
+
 #ifdef __cplusplus
 }
 #endif

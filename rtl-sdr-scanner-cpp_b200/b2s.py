@@ -77,6 +77,16 @@ class SignalEvent(C.Structure):
         return (self.kind, self.key, self.shift_hz, self.frame, self.time_ms, self.first_ms, self.last_ms)
 
 
+class AutoRecordAction(C.Structure):
+    """b2s_auto_record_action: what an auto-recording band did to its bank after one push (kind: REC_START / STOP / FLUSH / NONE_FREE)."""
+
+    _fields_ = [("kind", C.c_int32), ("channel", C.c_int32), ("shift_hz", C.c_int32), ("key", C.c_int32), ("frame", C.c_int64), ("from_frame", C.c_int64),
+                ("time_ms", C.c_int64), ("duration_ms", C.c_int64)]
+
+    def astuple(self):
+        return (self.kind, self.channel, self.shift_hz, self.key, self.frame, self.from_frame, self.time_ms, self.duration_ms)
+
+
 class Result(C.Structure):
     _fields_ = [
         ("n_transmissions", C.c_int32),
@@ -222,7 +232,10 @@ def lib():
         L.b2s_recorder_bank_history.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
         L.b2s_recorder_bank_start_from.argtypes = [C.c_void_p, C.c_int, C.c_int32, C.c_int64, C.c_int64]
         L.b2s_band_record_from.argtypes = [C.c_void_p, C.c_int, C.c_int32, C.c_int64]
-        for f in ("b2s_recorder_bank_set_history", "b2s_recorder_bank_history", "b2s_recorder_bank_start_from", "b2s_band_record_from"):
+        L.b2s_band_set_auto_record.argtypes = [C.c_void_p, C.c_int, C.c_int32]
+        L.b2s_band_get_auto_record_actions.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int)]
+        for f in ("b2s_recorder_bank_set_history", "b2s_recorder_bank_history", "b2s_recorder_bank_start_from", "b2s_band_record_from",
+                  "b2s_band_set_auto_record", "b2s_band_get_auto_record_actions"):
             getattr(L, f).restype = C.c_int
         for f in ("b2s_band", "b2s_recorder_bank"):
             getattr(L, f + "_save_state").argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -552,6 +565,18 @@ class Band(_Handle):
         """b2s_band_record_from: start `channel` of the attached bank at band frame `frame` (as in the signal events), from the bank's
         history, its chunks stamped with that frame's clock."""
         _check(lib().b2s_band_record_from(self._h, channel, shift_hz, frame))
+
+    def set_auto_record(self, enable: bool = True, preroll_frames: int = 0):
+        """b2s_band_set_auto_record: after each push the band starts and stops its attached bank's channels itself, as the reference's
+        SdrDevice::updateRecordings does, each recording from its transmission's START frame minus `preroll_frames`."""
+        _check(lib().b2s_band_set_auto_record(self._h, 1 if enable else 0, preroll_frames))
+
+    def auto_record_actions(self, cap: int = 65536, consume: bool = True):
+        """The oldest `cap` auto-record actions: [(kind, channel, shift_hz, key, frame, from_frame, time_ms, duration_ms)]."""
+        acts = (AutoRecordAction * max(cap, 1))()
+        count = C.c_int()
+        _check(lib().b2s_band_get_auto_record_actions(self._h, C.cast(acts, C.c_void_p), cap, 1 if consume else 0, C.byref(count)))
+        return [acts[i].astuple() for i in range(min(count.value, cap))]
 
     def save_state(self) -> bytes:
         """b2s_band_save_state: the band's whole state as an opaque snapshot (outstanding pushes are finished first)."""

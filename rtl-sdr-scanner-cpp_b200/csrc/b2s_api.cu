@@ -50,9 +50,9 @@ int fail(int code, const char* fmt, ...) {
     if (err__ != cudaSuccess) return fail(B2S_E_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(err__), __FILE__, __LINE__); \
   } while (0)
 
-// copies up to `cap` of the queued events to `out`, reports how many there are and drops the copied ones when asked to
-template <class Queue>
-static void hand_out_events(Queue& q, b2s_signal_event* out, int cap, int consume, int* count) {
+// copies up to `cap` of the queued events (or actions) to `out`, reports how many there are and drops the copied ones when asked to
+template <class Queue, class T>
+static void hand_out_events(Queue& q, T* out, int cap, int consume, int* count) {
   const int total = static_cast<int>(q.size()), n = out ? std::max(0, std::min(cap, total)) : 0;
   std::copy(q.begin(), q.begin() + n, out);
   *count = total;
@@ -675,9 +675,8 @@ struct b2s_recorder_bank {
   std::vector<Channel> ch;
   // History (b2s_recorder_bank_set_history): the newest hist_cap raw samples of the stream, stream position p in ring slot
   // p % hist_cap. hist_end counts the samples pushed since the last set_history or load; hist_epoch changes whenever the history is
-  // emptied, so that positions taken before are recognised as void. gather holds a catch-up piece whose samples (with the hc before
-  // it) wrap around the ring's end.
-  DevBuf<unsigned char> hist, gather;
+  // emptied, so that positions taken before are recognised as void.
+  DevBuf<unsigned char> hist;
   size_t hist_cap = 0;
   long long hist_end = 0;
   uint64_t hist_epoch = 0;
@@ -765,64 +764,74 @@ int bank_create(b2s_engine* e, int32_t sample_rate_hz, int32_t bandwidth_hz, int
   return 0;
 }
 
-// What a push of n_samples does: the recording channels (p.rec; only channel `only` when it is >= 0), each one's geometry in every
-// stage ([channel][stage], the return value) and output count (p.produced, p.most). Reads the channels' stream positions and changes
-// nothing.
-std::vector<StageChan> bank_plan(const b2s_recorder_bank* k, size_t n_samples, b2s_recorder_bank::Launched& p, int only = -1) {
-  const int n_st = static_cast<int>(k->stages.size());
-  p.rec.clear();
-  for (int i = 0; i < k->n_ch; ++i)
-    if (k->ch[i].recording && (only < 0 || i == only)) p.rec.push_back(i);
-  std::vector<StageChan> geo(p.rec.size() * n_st);
-  p.produced.assign(p.rec.size(), 0);
-  p.most = 0;
-  for (size_t i = 0; i < p.rec.size(); ++i) {
-    const auto& c = k->ch[p.rec[i]];
-    long long seen = c.seen, n_in = static_cast<long long>(n_samples);
-    for (int si = 0; si < n_st; ++si) {
-      const auto& st = k->stages[si];
-      StageChan& g = geo[i * n_st + si];
-      g.g0 = seen;
-      g.m0 = stage_outputs(seen, st.interp, st.decim);
-      g.n_in = static_cast<int>(n_in);
-      g.n_out = static_cast<int>(stage_outputs(seen + n_in, st.interp, st.decim) - g.m0);
-      g.phase_inc = si == 0 ? c.phase_inc : 0ull;
-      g.slot = p.rec[i];
-      seen = g.m0;
-      n_in = g.n_out;
-    }
-    p.produced[i] = n_in;
-    p.most = std::max(p.most, n_in);
+// Adds channel `channel`, fed its next n_samples stream samples, to the launch p: its geometry in every stage (appended to geo, which
+// is [channel][stage]) and its output count (p.produced, p.most). Reads the channel's stream position and changes nothing.
+void plan_channel(const b2s_recorder_bank* k, int channel, size_t n_samples, b2s_recorder_bank::Launched& p, std::vector<StageChan>& geo) {
+  const auto& c = k->ch[channel];
+  long long seen = c.seen, n_in = static_cast<long long>(n_samples);
+  for (size_t si = 0; si < k->stages.size(); ++si) {
+    const auto& st = k->stages[si];
+    StageChan g{};
+    g.g0 = seen;
+    g.m0 = stage_outputs(seen, st.interp, st.decim);
+    g.n_in = static_cast<int>(n_in);
+    g.n_out = static_cast<int>(stage_outputs(seen + n_in, st.interp, st.decim) - g.m0);
+    g.phase_inc = si == 0 ? c.phase_inc : 0ull;
+    g.slot = channel;
+    geo.push_back(g);
+    seen = g.m0;
+    n_in = g.n_out;
   }
+  p.rec.push_back(channel);
+  p.produced.push_back(n_in);
+  p.most = std::max(p.most, n_in);
+}
+
+// What a push of n_samples does: every recording channel (p.rec), each one's geometry in every stage ([channel][stage], the return
+// value) and output count (p.produced, p.most).
+std::vector<StageChan> bank_plan(const b2s_recorder_bank* k, size_t n_samples, b2s_recorder_bank::Launched& p) {
+  std::vector<StageChan> geo;
+  p.rec.clear();
+  p.produced.clear();
+  p.most = 0;
+  for (int i = 0; i < k->n_ch; ++i)
+    if (k->ch[i].recording) plan_channel(k, i, n_samples, p, geo);
   return geo;
 }
 
-// the history ring's slot of stream position pos (pos < 0 is the carry of a catch-up's first piece, which no kernel reads)
-size_t hist_slot(const b2s_recorder_bank* k, long long pos) {
-  const long long cap = static_cast<long long>(k->hist_cap);
-  return static_cast<size_t>((pos % cap + cap) % cap);
+// One stage launch: the polyphase kernel for a decimating stage, the general one otherwise
+template <class Args>
+int launch_stage(b2s_recorder_bank* k, const b2s_recorder_bank::Stage& st, const Args& a, int most_out) {
+  if (st.taps_pq.p) k_decimate_poly<<<((most_out + kPolyOut - 1) / kPolyOut) * a.n_ch, kPolyThreads, 0, k->stream>>>(a, st.taps_pq.p);
+  else k_resample<<<((most_out + a.per_cta - 1) / a.per_cta) * a.n_ch, kResampleThreads, sizeof(float2) * kResampleTile, k->stream>>>(a);
+  CU(cudaGetLastError());
+  return 0;
 }
+
+// the history ring's slot of stream position pos >= 0
+size_t hist_slot(const b2s_recorder_bank* k, long long pos) { return static_cast<size_t>(pos % static_cast<long long>(k->hist_cap)); }
 
 // The device half of a push whose n_samples input samples are on the device at `in`: one launch per stage (per kLaunchChannels
 // channels), the carries, and (p.fetch) the copy of the channels' int8 outputs into h_out[p.slot], all on the bank's stream. Advances the
-// channels' stream positions.
-// raw_carry == nullptr: the stream's next samples. Stage 0 reads the shared raw carry and moves it on, and the samples are appended to
-// the history; stage0_done (optional) is recorded once none of this reads `in` any more.
-// Otherwise a catch-up piece (bank_start_from) whose stage 0 finds the hc samples before `in` at raw_carry; the shared raw carry and
-// the history stay as they are.
-int bank_launch(b2s_recorder_bank* k, const void* in, const void* raw_carry, size_t n_samples, int64_t t0_ms, const std::vector<StageChan>& geo,
-                const b2s_recorder_bank::Launched& p, cudaEvent_t stage0_done) {
+// channels' stream positions by their stage-0 inputs.
+// ring0 == nullptr: the stream's next n_samples samples. Stage 0 reads the shared raw carry and moves it on, and the samples are
+// appended to the history; stage0_done (optional) is recorded once none of this reads `in` any more.
+// Otherwise a catch-up piece (bank_catch_up): stage 0 reads the history ring in place, channel p.rec[i] from ring slot ring0[i], with
+// the ring slots before it as its carry; `in` and n_samples are unused, and the shared raw carry and the history stay as they are.
+int bank_launch(b2s_recorder_bank* k, const void* in, size_t n_samples, int64_t t0_ms, const std::vector<StageChan>& geo, const b2s_recorder_bank::Launched& p,
+                cudaEvent_t stage0_done, const long long* ring0 = nullptr) {
   const int n_st = static_cast<int>(k->stages.size());
   const std::vector<int>& rec = p.rec;
   const int raw_kind = k->iq_format == B2S_IQ_CS8 ? 0 : 1;
-  const bool stream_push = raw_carry == nullptr;
+  const bool stream_push = ring0 == nullptr;
+  int rc;
   for (int si = 0; si < n_st; ++si) {
     auto& st = k->stages[si];
     const bool last = si + 1 == n_st;
     for (size_t c0 = 0; c0 < rec.size(); c0 += kLaunchChannels) {
       ResampleArgs a{};
       a.in = si == 0 ? in : static_cast<const void*>(st.buf.p + st.hc);
-      a.carry = si > 0 ? static_cast<const void*>(st.buf.p) : stream_push ? static_cast<const void*>(k->carry_raw.p) : raw_carry;
+      a.carry = si > 0 ? static_cast<const void*>(st.buf.p) : stream_push ? static_cast<const void*>(k->carry_raw.p) : nullptr;
       a.in_stride = si == 0 ? 0 : static_cast<long long>(st.stride);
       a.kind = si == 0 ? raw_kind : 2;
       a.iq_scale = k->iq_scale;
@@ -845,12 +854,15 @@ int bank_launch(b2s_recorder_bank* k, const void* in, const void* raw_carry, siz
         a.ch[j] = geo[(c0 + j) * n_st + si];
         most_out = std::max(most_out, a.ch[j].n_out);
       }
-      if (most_out > 0 && st.taps_pq.p) {  // decimating stage: polyphase kernel
-        k_decimate_poly<<<((most_out + kPolyOut - 1) / kPolyOut) * a.n_ch, kPolyThreads, 0, k->stream>>>(a, st.taps_pq.p);
-        CU(cudaGetLastError());
-      } else if (most_out > 0) {
-        k_resample<<<((most_out + a.per_cta - 1) / a.per_cta) * a.n_ch, kResampleThreads, sizeof(float2) * kResampleTile, k->stream>>>(a);
-        CU(cudaGetLastError());
+      if (most_out > 0 && si == 0 && !stream_push) {
+        RingArgs r{};
+        static_cast<ResampleArgs&>(r) = a;
+        r.in = k->hist.p;
+        r.ring_cap = static_cast<long long>(k->hist_cap);
+        for (int j = 0; j < a.n_ch; ++j) r.ring0[j] = ring0[c0 + j];
+        if ((rc = launch_stage(k, st, r, most_out))) return rc;
+      } else if (most_out > 0 && (rc = launch_stage(k, st, a, most_out))) {
+        return rc;
       }
       // carry the newest inputs of this stage over to the next push
       if (si > 0) {
@@ -880,13 +892,13 @@ int bank_launch(b2s_recorder_bank* k, const void* in, const void* raw_carry, siz
     const size_t rows = static_cast<size_t>(rec.back()) + 1, pitch = 2 * k->out_stride;
     CU(cudaMemcpy2DAsync(k->h_out[p.slot].p, pitch, k->d_out.p, pitch, 2 * static_cast<size_t>(p.most), rows, cudaMemcpyDeviceToHost, k->stream));
   }
-  for (int r : rec) {
-    auto& c = k->ch[r];
+  for (size_t i = 0; i < rec.size(); ++i) {
+    auto& c = k->ch[rec[i]];
     if (!c.timed) {
       c.timed = true;
       c.start_ms = t0_ms;
     }
-    c.seen += static_cast<long long>(n_samples);
+    c.seen += geo[i * n_st].n_in;
   }
   return 0;
 }
@@ -935,7 +947,7 @@ int bank_push(b2s_recorder_bank* k, const void* iq, size_t n_samples, int64_t t0
     in = k->staging.p;
   }
   p.fetch = p.most > 0 && (out_iq || k->keep_chunks);
-  if ((rc = bank_launch(k, in, nullptr, n_samples, t0_ms, geo, p, nullptr))) return rc;
+  if ((rc = bank_launch(k, in, n_samples, t0_ms, geo, p, nullptr))) return rc;
   CU(cudaStreamSynchronize(k->stream));
   bank_take(k, p, out_iq, cap_samples, n_out);
   return 0;
@@ -954,7 +966,7 @@ int bank_feed(b2s_recorder_bank* k, const void* in, size_t n_samples, int64_t t0
   p.slot = k->has_pending ? k->pending.slot ^ 1 : 0;
   p.fetch = p.most > 0;
   CU(cudaStreamWaitEvent(k->stream, ready, 0));
-  rc = bank_launch(k, in, nullptr, n_samples, t0_ms, geo, p, stage0_done);
+  rc = bank_launch(k, in, n_samples, t0_ms, geo, p, stage0_done);
   if (rc) return rc;
   CU(cudaEventRecord(k->out_ready[p.slot], k->stream));
   if ((rc = bank_settle(k))) return rc;
@@ -963,40 +975,59 @@ int bank_feed(b2s_recorder_bank* k, const void* in, size_t n_samples, int64_t t0
   return 0;
 }
 
-// Start `channel` at stream position `position` of the history (b2s_recorder_bank_start_from): the samples [position, end) run through
-// the channel alone at once, cut every max_in samples from `position` as a fresh bank's pushes would be, with seen counting from
-// `position`. Stage 0 reads each piece in the ring, with the hc samples before it as its carry (the first piece reads none: they
-// precede the channel's start); a piece whose span [start - hc, end) wraps around the ring's end is gathered first. Synchronous on
-// the bank's stream, which also orders it after every piece a band has fed.
+// A channel to start from the history: b2s_recorder_bank_start_from's arguments
+struct CatchUp {
+  int channel;
+  int32_t shift_hz;
+  long long position;
+  int64_t start_ms;
+};
+
+// Start the channels `starts` (idle, distinct, positions inside the history) at their positions: each channel's samples [position, end)
+// run at once, cut every max_in samples from its own position as a fresh bank's pushes would be, with seen counting from that position.
+// Piece j of every channel goes into one launch per stage (per kLaunchChannels channels), each channel with its own geometry; channels
+// with fewer pieces drop out of the later launches. Stage 0 reads each piece in the history ring in place, with the ring slots before it
+// as its carry (the first piece reads none: they precede the channel's start). One synchronise per piece index. Synchronous on the
+// bank's stream, which also orders it after every piece a band has fed; the caller has settled the bank's pending piece.
+int bank_catch_up(b2s_recorder_bank* k, std::vector<CatchUp> starts) {
+  std::sort(starts.begin(), starts.end(), [](const CatchUp& a, const CatchUp& b) { return a.channel < b.channel; });  // rows of one copy
+  for (const CatchUp& s : starts) {
+    auto& c = k->ch[s.channel];
+    start_channel(c, rotator_phase_inc(s.shift_hz, k->sample_rate));
+    if (s.position < k->hist_end) {  // stamped from start_ms by its first piece (at the end of the history: by the next push)
+      c.timed = true;
+      c.start_ms = s.start_ms;
+    }
+  }
+  CU(cudaSetDevice(k->engine->device));
+  const long long step = static_cast<long long>(k->max_in);
+  for (long long j = 0;; ++j) {
+    b2s_recorder_bank::Launched p;
+    std::vector<StageChan> geo;
+    std::vector<long long> ring0;
+    for (const CatchUp& s : starts) {
+      const long long a = s.position + j * step;
+      if (a >= k->hist_end) continue;
+      plan_channel(k, s.channel, static_cast<size_t>(std::min(step, k->hist_end - a)), p, geo);
+      ring0.push_back(static_cast<long long>(hist_slot(k, a)));
+    }
+    if (p.rec.empty()) return 0;
+    p.fetch = p.most > 0;
+    int rc = bank_launch(k, nullptr, 0, 0, geo, p, nullptr, ring0.data());
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(k->stream));
+    bank_take(k, p, nullptr, 0, nullptr);
+  }
+}
+
+// b2s_recorder_bank_start_from: the checks, then the catch-up of the one channel
 int bank_start_from(b2s_recorder_bank* k, int channel, int32_t shift_hz, long long position, int64_t start_ms, const char* who) {
   int rc = bank_settle(k);
   if (rc) return rc;
   if (k->ch[channel].recording) return fail(B2S_E_STATE, "%s: channel %d is already recording", who, channel);
   if (!k->hist_cap || position < k->hist_oldest() || position > k->hist_end)
     return fail(B2S_E_INVALID, "%s: position %lld is outside the history [%lld, %lld)", who, position, k->hist_oldest(), k->hist_end);
-  CU(cudaSetDevice(k->engine->device));
-  start_channel(k->ch[channel], rotator_phase_inc(shift_hz, k->sample_rate));
-  const size_t bps = k->raw_bytes(), hc = static_cast<size_t>(k->stages[0].hc);
-  for (long long s = position; s < k->hist_end; s += static_cast<long long>(k->max_in)) {
-    const size_t n = static_cast<size_t>(std::min<long long>(static_cast<long long>(k->max_in), k->hist_end - s));
-    const size_t at = hist_slot(k, s);
-    const unsigned char* in = k->hist.p + at * bps;
-    if (at < hc || at + n > k->hist_cap) {
-      for (size_t done = 0; done < hc + n;) {
-        const size_t from = hist_slot(k, s - static_cast<long long>(hc - done)), m = std::min(hc + n - done, k->hist_cap - from);
-        CU(cudaMemcpyAsync(k->gather.p + done * bps, k->hist.p + from * bps, m * bps, cudaMemcpyDeviceToDevice, k->stream));
-        done += m;
-      }
-      in = k->gather.p + hc * bps;
-    }
-    b2s_recorder_bank::Launched p;
-    const std::vector<StageChan> geo = bank_plan(k, n, p, channel);
-    p.fetch = p.most > 0;
-    if ((rc = bank_launch(k, in, in - hc * bps, n, start_ms, geo, p, nullptr))) return rc;
-    CU(cudaStreamSynchronize(k->stream));
-    bank_take(k, p, nullptr, 0, nullptr);
-  }
-  return 0;
+  return bank_catch_up(k, {CatchUp{channel, shift_hz, position, start_ms}});
 }
 
 // Detach the band's bank (b->mutex held): the band's outstanding pushes are drained and the bank's last push settled, so that neither
@@ -1008,6 +1039,7 @@ int band_detach(b2s_band* b) {
   const int rc2 = bank_settle(b->bank);
   b->bank->band = nullptr;
   b->bank = nullptr;
+  b->autorec = b2s_band::AutoRecord{};
   b->d_whole = DevBuf<unsigned char>();
   return rc ? rc : rc2;
 }
@@ -1028,6 +1060,89 @@ int band_feed(b2s_band* b, const void* in, int64_t frame, size_t first, size_t f
   const long long stride = b->cfg.frame_stride_samples;
   while (!b->hist_pieces.empty() && b->hist_pieces.front().position + b->hist_pieces.front().n_frames * stride <= k->hist_oldest()) b->hist_pieces.pop_front();
   return 0;
+}
+
+// Band frame `frame`'s position in the attached bank's stream and its clock, when the bank's history holds it: b2s_band_record_from's rule
+bool band_frame_in_history(const b2s_band* b, int64_t frame, long long* position, int64_t* time_ms) {
+  const b2s_recorder_bank* k = b->bank;
+  if (!k || !k->hist_cap || b->hist_epoch != k->hist_epoch) return false;
+  const b2s_band::HistPiece* piece = nullptr;  // the newest piece that starts at or before `frame`
+  for (auto it = b->hist_pieces.rbegin(); it != b->hist_pieces.rend() && !piece; ++it)
+    if (it->frame <= frame) piece = &*it;
+  if (!piece || frame >= piece->frame + piece->n_frames) return false;
+  *position = piece->position + (frame - piece->frame) * static_cast<long long>(b->cfg.frame_stride_samples);
+  *time_ms = host::frame_time(piece->t0_ms, piece->period_ms, piece->first + static_cast<size_t>(frame - piece->frame));
+  return *position >= k->hist_oldest();
+}
+
+// The oldest band frame band_frame_in_history accepts, or -1 when it accepts none
+int64_t band_oldest_frame(const b2s_band* b) {
+  const b2s_recorder_bank* k = b->bank;
+  if (!k || !k->hist_cap || b->hist_epoch != k->hist_epoch) return -1;
+  const long long stride = b->cfg.frame_stride_samples;
+  for (const auto& p : b->hist_pieces) {
+    const long long skip = std::max(0LL, (k->hist_oldest() - p.position + stride - 1) / stride);  // frames of the piece that left
+    if (skip < p.n_frames) return p.frame + skip;
+  }
+  return -1;
+}
+
+bool bank_auto_recorded(const b2s_recorder_bank* k) { return k->band && k->band->autorec.on; }
+
+// Auto-record's decision for the push that finished last (b->autorec.due): ScanPolicy::update_recordings on the mailbox, then the bank's
+// stops, the starts without usable history, and one catch-up for the starts from history, in that order of effect on the bank (each
+// action touches another channel, so the order does not show in the output).
+int band_auto_decide(b2s_band* b) {
+  auto& a = b->autorec;
+  if (!a.on || !a.due) return 0;
+  a.due = false;
+  b2s_recorder_bank* k = b->bank;
+  std::vector<b2s_transmission> list;
+  {
+    std::lock_guard<std::mutex> lk(b->qmutex);
+    list = b->mailbox;
+  }
+  std::vector<b2s_recorder_action> acts;
+  std::vector<int> source;
+  a.policy->update_recordings(a.time_ms, list.data(), static_cast<int>(list.size()), acts, &source);
+  int rc = bank_settle(k);
+  if (rc) return rc;
+  const int64_t oldest = band_oldest_frame(b);
+  std::vector<CatchUp> catch_up;
+  for (size_t i = 0; i < acts.size(); ++i) {
+    const b2s_recorder_action& act = acts[i];
+    b2s_auto_record_action out{act.kind, act.recorder, act.shift_hz, source[i] >= 0 ? list[source[i]].key : 0, a.frame, -1, a.time_ms, 0};
+    if (act.kind == B2S_REC_STOP) {
+      out.key = a.key[act.recorder];
+      out.duration_ms = act.duration_ms;
+      auto& c = k->ch[act.recorder];
+      c.recording = false;
+      c.drop();
+    } else if (act.kind == B2S_REC_START) {
+      a.key[act.recorder] = out.key;
+      bool found = false;
+      std::pair<int64_t, int64_t> start{0, 0};
+      {
+        std::lock_guard<std::mutex> lk(b->qmutex);
+        auto it = b->start_of.find(out.key);
+        found = it != b->start_of.end() && it->second.first > b->start_lost_through;
+        if (found) start = it->second;
+      }
+      long long position = 0;
+      int64_t time_ms = 0;
+      found = found && start.first >= a.enabled_at && start.first <= a.frame && oldest >= 0 && start.first >= oldest &&
+              band_frame_in_history(b, start.first, &position, &time_ms);
+      if (found) {
+        out.from_frame = std::max(start.first - a.preroll, oldest);
+        band_frame_in_history(b, out.from_frame, &position, &out.time_ms);
+        catch_up.push_back(CatchUp{act.recorder, act.shift_hz, position, out.time_ms});
+      } else {
+        start_channel(k->ch[act.recorder], rotator_phase_inc(act.shift_hz, k->sample_rate));
+      }
+    }
+    b->auto_actions.push_back(out);
+  }
+  return bank_catch_up(k, std::move(catch_up));
 }
 
 // ---- recorder bank snapshot: the raw-sample carry, then per channel its position, its rows of the stages' carries and its chunks ----
@@ -1301,11 +1416,7 @@ int b2s_band_set_stream(b2s_band* b, void* cuda_stream) {
   return 0;
 }
 
-int b2s_band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, double frame_period_ms, b2s_result* out) {
-  if (!b || (!iq && n_frames)) return fail(B2S_E_INVALID, "NULL argument");
-  std::lock_guard<std::mutex> lock(b->mutex);
-  CU(cudaSetDevice(b->engine->device));
-  if (b->async_mode && out) return fail(B2S_E_INVALID, "with B2S_FLAG_ASYNC results are collected by b2s_band_sync; pass out = NULL to b2s_band_push");
+static int band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, double frame_period_ms, b2s_result* out) {
   if (out) {
     out->n_transmissions = 0;
     out->n_transmissions_total = 0;
@@ -1442,12 +1553,31 @@ int b2s_band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, d
   return 0;
 }
 
+int b2s_band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms, double frame_period_ms, b2s_result* out) {
+  if (!b || (!iq && n_frames)) return fail(B2S_E_INVALID, "NULL argument");
+  std::lock_guard<std::mutex> lock(b->mutex);
+  CU(cudaSetDevice(b->engine->device));
+  if (b->async_mode && out) return fail(B2S_E_INVALID, "with B2S_FLAG_ASYNC results are collected by b2s_band_sync; pass out = NULL to b2s_band_push");
+  int rc = 0;
+  if (b->autorec.due) {  // an asynchronous band's previous push: decided before this push feeds the bank
+    if ((rc = b->drain()) || (rc = band_auto_decide(b))) return rc;
+  }
+  const int64_t frame0 = b->frames_pushed;
+  if ((rc = band_push(b, iq, n_frames, t0_ms, frame_period_ms, out))) return rc;
+  if (!b->autorec.on || n_frames == 0) return 0;
+  b->autorec.due = true;
+  b->autorec.frame = frame0 + static_cast<int64_t>(n_frames) - 1;
+  b->autorec.time_ms = host::frame_time(t0_ms, frame_period_ms, n_frames - 1);
+  return b->async_mode ? 0 : band_auto_decide(b);
+}
+
 int b2s_band_sync(b2s_band* b, b2s_result* out) {
   if (!b) return fail(B2S_E_INVALID, "NULL band");
   std::lock_guard<std::mutex> lock(b->mutex);
   CU(cudaSetDevice(b->engine->device));
   int rc = b->drain();
   if (rc) return rc;
+  if ((rc = band_auto_decide(b))) return rc;
   if (b->bank && (rc = bank_settle(b->bank))) return rc;
   if (out) {
     out->n_transmissions_total = static_cast<int32_t>(b->mailbox.size());
@@ -1599,7 +1729,12 @@ int b2s_band_load_state(b2s_band* b, const void* buf, size_t len) {
   std::lock_guard<std::mutex> lock(b->mutex);
   CU(cudaSetDevice(b->engine->device));
   const int rc = b->load_state(buf, len);
-  if (!rc) b->hist_pieces.clear();  // the frames pushed before belong to another stream
+  if (!rc) {  // the frames pushed before belong to another stream
+    b->hist_pieces.clear();
+    b->autorec = b2s_band::AutoRecord{};
+    std::lock_guard<std::mutex> lk(b->qmutex);
+    b->start_of.clear();
+  }
   return rc;
 }
 
@@ -1610,22 +1745,57 @@ int b2s_band_record_from(b2s_band* b, int channel, int32_t shift_hz, int64_t fra
   b2s_recorder_bank* k = b->bank;
   if (!k || !k->hist_cap) return fail(B2S_E_INVALID, "%s: the band has no recorder bank that keeps history", who);
   if (channel < 0 || channel >= k->n_ch) return fail(B2S_E_INVALID, "%s: bad channel", who);
-  const b2s_band::HistPiece* piece = nullptr;  // the newest piece that starts at or before `frame`
-  if (b->hist_epoch == k->hist_epoch) {
-    for (auto it = b->hist_pieces.rbegin(); it != b->hist_pieces.rend() && !piece; ++it)
-      if (it->frame <= frame) piece = &*it;
-  }
-  const long long position = piece ? piece->position + (frame - piece->frame) * static_cast<long long>(b->cfg.frame_stride_samples) : 0;
-  if (!piece || frame >= piece->frame + piece->n_frames || position < k->hist_oldest())
+  if (b->autorec.on) return fail(B2S_E_STATE, "%s: the band records automatically (b2s_band_set_auto_record)", who);
+  long long position = 0;
+  int64_t time_ms = 0;
+  if (!band_frame_in_history(b, frame, &position, &time_ms))
     return fail(B2S_E_INVALID, "%s: frame %lld is not in the recorder bank's history", who, static_cast<long long>(frame));
-  return bank_start_from(k, channel, shift_hz, position, host::frame_time(piece->t0_ms, piece->period_ms, piece->first + static_cast<size_t>(frame - piece->frame)), who);
+  return bank_start_from(k, channel, shift_hz, position, time_ms, who);
+}
+
+int b2s_band_set_auto_record(b2s_band* b, int enable, int32_t preroll_frames) {
+  const char* who = "b2s_band_set_auto_record";
+  if (!b || preroll_frames < 0) return fail(B2S_E_INVALID, "%s: bad argument", who);
+  std::lock_guard<std::mutex> lock(b->mutex);
+  auto& a = b->autorec;
+  if (!enable) {
+    a = b2s_band::AutoRecord{};
+    return 0;
+  }
+  b2s_recorder_bank* k = b->bank;
+  if (!k) return fail(B2S_E_INVALID, "%s: the band has no recorder bank", who);
+  if (a.on) {
+    a.preroll = preroll_frames;
+    return 0;
+  }
+  CU(cudaSetDevice(b->engine->device));
+  const int rc = bank_settle(k);
+  if (rc) return rc;
+  for (int i = 0; i < k->n_ch; ++i)
+    if (k->ch[i].recording) return fail(B2S_E_STATE, "%s: channel %d of the bank is recording", who, i);
+  a.policy = std::make_unique<host::ScanPolicy>(nullptr, nullptr, 0, k->sample_rate, k->n_ch, 0);
+  a.key.assign(k->n_ch, 0);
+  a.preroll = preroll_frames;
+  a.enabled_at = b->frames_pushed;
+  a.on = true;
+  std::lock_guard<std::mutex> lk(b->qmutex);
+  b->start_of.clear();
+  b->start_lost_through = -1;
+  return 0;
+}
+
+int b2s_band_get_auto_record_actions(b2s_band* b, b2s_auto_record_action* out, int cap, int consume, int* count) {
+  if (!b || !count) return fail(B2S_E_INVALID, "b2s_band_get_auto_record_actions: NULL argument");
+  std::lock_guard<std::mutex> lock(b->mutex);
+  hand_out_events(b->auto_actions, out, cap, consume, count);
+  return 0;
 }
 
 int b2s_band_set_event_log(b2s_band* b, int enable) {
   if (!b) return fail(B2S_E_INVALID, "NULL band");
   std::lock_guard<std::mutex> lock(b->mutex);
   b->event_log = enable != 0;
-  if (!b->event_log) {  // the slots' record buffers go once no chunk in flight writes them
+  if (!b->event_log && !b->autorec.on) {  // the slots' record buffers go once no chunk in flight writes them
     CU(cudaSetDevice(b->engine->device));
     int rc = b->drain();
     if (rc) return rc;
@@ -1903,6 +2073,7 @@ int b2s_recorder_bank_destroy(b2s_recorder_bank* k) {
 }
 int b2s_recorder_bank_start(b2s_recorder_bank* k, int channel, int32_t shift_hz) {
   if (!k || channel < 0 || channel >= k->n_ch) return fail(B2S_E_INVALID, "b2s_recorder_bank_start: bad channel");
+  if (bank_auto_recorded(k)) return fail(B2S_E_STATE, "b2s_recorder_bank_start: the bank's band records automatically (b2s_band_set_auto_record)");
   const int rc = bank_settle(k);  // a push an asynchronous band left pending belongs to the recording as it was
   if (rc) return rc;
   if (k->ch[channel].recording) return fail(B2S_E_STATE, "b2s_recorder_bank_start: channel %d is already recording", channel);
@@ -1911,6 +2082,7 @@ int b2s_recorder_bank_start(b2s_recorder_bank* k, int channel, int32_t shift_hz)
 }
 int b2s_recorder_bank_stop(b2s_recorder_bank* k, int channel) {
   if (!k || channel < 0 || channel >= k->n_ch) return fail(B2S_E_INVALID, "b2s_recorder_bank_stop: bad channel");
+  if (bank_auto_recorded(k)) return fail(B2S_E_STATE, "b2s_recorder_bank_stop: the bank's band records automatically (b2s_band_set_auto_record)");
   const int rc = bank_settle(k);
   if (rc) return rc;
   auto& c = k->ch[channel];
@@ -1967,15 +2139,14 @@ int b2s_recorder_bank_set_history(b2s_recorder_bank* k, size_t samples) {
   if (rc) return rc;
   CU(cudaSetDevice(k->engine->device));
   CU(cudaStreamSynchronize(k->stream));
-  const size_t bps = k->raw_bytes(), hc = static_cast<size_t>(k->stages[0].hc);
-  if (samples > (SIZE_MAX / bps) - k->max_in - hc) return fail(B2S_E_NOMEM, "b2s_recorder_bank_set_history: %zu samples do not fit in memory", samples);
-  DevBuf<unsigned char> ring, gather;  // allocated before anything changes: a refusal keeps the previous history
-  if (samples && ((rc = ring.alloc(samples * bps)) || (rc = gather.alloc((k->max_in + hc) * bps)))) {
+  const size_t bps = k->raw_bytes();
+  if (samples > SIZE_MAX / bps) return fail(B2S_E_NOMEM, "b2s_recorder_bank_set_history: %zu samples do not fit in memory", samples);
+  DevBuf<unsigned char> ring;  // allocated before anything changes: a refusal keeps the previous history
+  if (samples && (rc = ring.alloc(samples * bps))) {
     cudaGetLastError();  // the failed allocation is not an error of later calls
     return rc;
   }
   k->hist = std::move(ring);
-  k->gather = std::move(gather);
   k->hist_cap = samples;
   k->hist_end = 0;
   ++k->hist_epoch;
@@ -1989,6 +2160,7 @@ int b2s_recorder_bank_history(b2s_recorder_bank* k, int64_t* oldest, int64_t* en
 }
 int b2s_recorder_bank_start_from(b2s_recorder_bank* k, int channel, int32_t shift_hz, int64_t position, int64_t start_ms) {
   if (!k || channel < 0 || channel >= k->n_ch) return fail(B2S_E_INVALID, "b2s_recorder_bank_start_from: bad channel");
+  if (bank_auto_recorded(k)) return fail(B2S_E_STATE, "b2s_recorder_bank_start_from: the bank's band records automatically (b2s_band_set_auto_record)");
   return bank_start_from(k, channel, shift_hz, position, start_ms, "b2s_recorder_bank_start_from");
 }
 

@@ -58,6 +58,7 @@ struct PushSlot {
   PinBuf<TrackResult> h_result;
   DevBuf<TrackEvent> d_log;  // [N] the signal event records of the chunk's K4 (TrackArgs::log); allocated while the log is on
   bool log_on = false;       // the event log was on when the chunk was enqueued
+  bool log_starts = false;   // auto-record was on: K4 logs even with the event log off, and the STARTs go to the band's start_of
   int64_t frame_base = 0;    // frames pushed to the band before the chunk's first
   Event sorted_done, tev[2];
   bool host_track = false;  // this chunk's bookkeeping runs on the host (the caller asked for every frame's list)
@@ -126,6 +127,23 @@ struct b2s_band : public DeviceQueries {
   };
   std::deque<HistPiece> hist_pieces;
   uint64_t hist_epoch = 0;
+  // Auto-record (b2s_band_set_auto_record): after each push the band runs the reference's recorder assignment on the push's mailbox and
+  // starts and stops the attached bank's channels itself. `policy` holds the recorders' state; `key` the map key each channel was started
+  // for; `due` marks a push whose decision has not run yet (its last frame and that frame's clock in frame, time_ms).
+  struct AutoRecord {
+    bool on = false;
+    int32_t preroll = 0;
+    int64_t enabled_at = 0;  // frames_pushed when it was enabled: START records of earlier frames are not used
+    std::unique_ptr<host::ScanPolicy> policy;
+    std::vector<int32_t> key;
+    bool due = false;
+    int64_t frame = 0, time_ms = 0;
+  } autorec;
+  std::deque<b2s_auto_record_action> auto_actions;  // not yet collected by b2s_band_get_auto_record_actions
+  // The latest START record of each key from the device log (or the host tracker's) while auto-record is on, as (band frame, clock), and
+  // the last frame of the newest chunk whose device log lost records (guarded by qmutex: the worker writes them)
+  std::map<int32_t, std::pair<int64_t, int64_t>> start_of;
+  int64_t start_lost_through = -1;
   int max_frames = 0;
   int slot_capacity = 0;  // detection entries per frame
   int detect_bins = kDetectBinsPerCta;  // bins per K2 CTA (DetectArgs::bins_per_cta)
@@ -966,8 +984,9 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
   s.epoch = reset_epoch;
   s.host_track = out && out->frame_tx_count;  // every frame's list is wanted: the bookkeeping runs on the host (tracker.h)
   s.log_on = event_log;
+  s.log_starts = autorec.on;
   s.frame_base = frames_pushed;
-  if (s.log_on && !s.host_track && (rc = s.d_log.alloc(n))) return rc;
+  if ((s.log_on || s.log_starts) && !s.host_track && (rc = s.d_log.alloc(n))) return rc;
   if (s.host_track && (rc = state_to_host_tracker())) return rc;
   s.dense_q_on = out && out->noise_sub_db;
   s.dense_avg_on = out && out->avg_db;
@@ -1198,7 +1217,7 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
     ta.tx = s.d_tx.p;
     ta.hit = d_track_hit.p;
     ta.sort_keys = d_track_sort.p;
-    ta.log = s.log_on ? s.d_log.p : nullptr;
+    ta.log = s.log_on || s.log_starts ? s.d_log.p : nullptr;
     ta.log_cap = n;
     // k_track runs the push unless it would pass its shared tables; then it leaves the map untouched and sets the result's
     // hand-off flag, and k_track_wide, always enqueued behind it, runs the push from the same map. Otherwise k_track_wide exits.
@@ -1292,14 +1311,21 @@ int b2s_band::finish_chunk(PushSlot& s) {
       std::lock_guard<std::mutex> lk(qmutex);
       if (s.epoch == reset_epoch) mailbox.swap(list);  // (a reset issued after this chunk was enqueued has emptied the mailbox: keep it so)
     }
-    if (s.log_on && r.n_log > 0) {  // the chunk's signal events: in-launch frames become frames of the band
+    if ((s.log_on || s.log_starts) && r.n_log > 0) {  // the chunk's signal events: in-launch frames become frames of the band
       std::vector<TrackEvent> rec(std::min(r.n_log, n));
       CU(cudaMemcpyAsync(rec.data(), s.d_log.p, sizeof(TrackEvent) * rec.size(), cudaMemcpyDeviceToHost, st));
       CU(cudaStreamSynchronize(st));
       prof.d2h_bytes += sizeof(TrackEvent) * rec.size();
       std::lock_guard<std::mutex> lk(qmutex);
-      for (const TrackEvent& e : rec) events.push_back(b2s_signal_event{e.kind, e.key, e.shift_hz, 0, s.frame_base + e.frame, e.time, e.first, e.last});
-      if (r.n_log > n) events.push_back(b2s_signal_event{B2S_EV_LOST, r.n_log - n, 0, 0, events.back().frame, events.back().time_ms, 0, 0});
+      if (s.log_on) {
+        for (const TrackEvent& e : rec) events.push_back(b2s_signal_event{e.kind, e.key, e.shift_hz, 0, s.frame_base + e.frame, e.time, e.first, e.last});
+        if (r.n_log > n) events.push_back(b2s_signal_event{B2S_EV_LOST, r.n_log - n, 0, 0, events.back().frame, events.back().time_ms, 0, 0});
+      }
+      if (s.log_starts) {
+        for (const TrackEvent& e : rec)
+          if (e.kind == B2S_EV_START) start_of[e.key] = {s.frame_base + e.frame, e.time};
+        if (r.n_log > n) start_lost_through = s.frame_base + T - 1;  // a later START of any key may be among the lost
+      }
     }
     if (profiling && s.tev[0]) {
       float ms = 0.0f;
@@ -1331,14 +1357,18 @@ int b2s_band::finish_chunk(PushSlot& s) {
     tracker.p.center = s.center;
     Tracker::Watch watch{s.n_watch, s.watch_key, s.h_watch_max.p, s.h_cand_flag.p};
     std::vector<b2s_signal_event> logged;
-    tracker.log = s.log_on ? &logged : nullptr;
+    tracker.log = s.log_on || s.log_starts ? &logged : nullptr;
     tracker.log_frame_base = s.frame_base;
     rc = tracker.run(s.h_entries.p, h_off, T, s.t0_ms, s.period_ms, s.frame_offset, *this, true, watch, states);
     tracker.log = nullptr;
     if (rc) return rc;
     if (!logged.empty()) {
       std::lock_guard<std::mutex> lk(qmutex);
-      events.insert(events.end(), logged.begin(), logged.end());
+      if (s.log_on) events.insert(events.end(), logged.begin(), logged.end());
+      if (s.log_starts) {
+        for (const b2s_signal_event& e : logged)
+          if (e.kind == B2S_EV_START) start_of[e.key] = {e.frame, e.time_ms};
+      }
     }
     prof.tracker_host_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
     // the mailbox after the last frame of this chunk (Notification::notify, transmission.cpp:67)

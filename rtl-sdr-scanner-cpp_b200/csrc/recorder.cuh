@@ -18,6 +18,7 @@
 // sdr_device.cpp:39-41): every channel runs the same stages on the same stream, each with its own shift, start and buffers. CTA b
 // works for channel b % n_ch, so the CTAs of all channels that cover the same span of the stream are adjacent in launch order. In
 // the first stage they read the same raw samples: one read from HBM, the others from L2. A stand-alone recorder is a bank of one.
+// A catch-up (a recording started from the bank's history) runs the same kernels with RingArgs: stage 0 reads the history ring in place.
 #pragma once
 #include <cmath>
 #include <vector>
@@ -57,6 +58,14 @@ struct ResampleArgs {
   StageChan ch[kLaunchChannels];
 };
 
+// Stage 0 of a catch-up: the raw samples come from the bank's history ring. `in` is the ring's base; the carry is the ring itself (the hc
+// samples before a piece are the ring slots before it), so `carry` and `in_stride` are unused. Launch channel j's sample g0 sits in ring
+// slot ring0[j]. Kept out of ResampleArgs so that the stream pushes' launches and kernels stay as they are.
+struct RingArgs : ResampleArgs {
+  long long ring_cap;  // capacity in samples
+  long long ring0[kLaunchChannels];
+};
+
 // what one CTA reads: its channel's view of the stage input
 struct StageView {
   const void* in;
@@ -65,9 +74,19 @@ struct StageView {
   int n_in, hc, kind;
   float iq_scale;
 };
-__device__ __forceinline__ StageView stage_view(const ResampleArgs& a, const StageChan& c) {
+__device__ __forceinline__ StageView stage_view(const ResampleArgs& a, const StageChan& c, int) {
   const long long off = static_cast<long long>(c.slot) * a.in_stride * (a.kind == 0 ? 2 : 8);
   return StageView{static_cast<const char*>(a.in) + off, static_cast<const char*>(a.carry) + off, c.g0, c.n_in, a.hc, a.kind, a.iq_scale};
+}
+struct RingView {
+  const void* ring;
+  long long cap, at0;  // at0: the ring slot of sample g0
+  long long g0;
+  int n_in, kind;
+  float iq_scale;
+};
+__device__ __forceinline__ RingView stage_view(const RingArgs& a, const StageChan& c, int j) {
+  return RingView{a.in, a.ring_cap, a.ring0[j], c.g0, c.n_in, a.kind, a.iq_scale};
 }
 
 // sample g of this stage's input stream, before the rotator (zero before startRecording)
@@ -83,6 +102,21 @@ __device__ __forceinline__ float2 resample_raw(const StageView& a, long long g) 
   const float2* p = rel >= 0 ? static_cast<const float2*>(a.in) + rel : static_cast<const float2*>(a.carry) + (a.hc + rel);
   return *p;
 }
+// The same from the ring: every sample read is at [piece start - hc, end of the history), inside the history's window of ring_cap samples
+// that also holds the piece's start, so rel lies in (-cap, cap) and one wrap in either direction takes the slot modulo the capacity.
+__device__ __forceinline__ float2 resample_raw(const RingView& a, long long g) {
+  if (g < 0) return make_float2(0.0f, 0.0f);
+  const long long rel = g - a.g0;
+  if (rel >= a.n_in) return make_float2(0.0f, 0.0f);
+  long long i = a.at0 + rel;
+  if (i < 0) i += a.cap;
+  else if (i >= a.cap) i -= a.cap;
+  if (a.kind == 0) {
+    const char2 s = static_cast<const char2*>(a.ring)[i];
+    return make_float2(static_cast<float>(s.x) * a.iq_scale, static_cast<float>(s.y) * a.iq_scale);
+  }
+  return static_cast<const float2*>(a.ring)[i];
+}
 // exp(i * 2 pi * turns), turns as a 64-bit binary fraction
 __device__ __forceinline__ float2 rotor_of(unsigned long long turns64) {
   float sn, cs;
@@ -90,7 +124,8 @@ __device__ __forceinline__ float2 rotor_of(unsigned long long turns64) {
   return make_float2(cs, sn);
 }
 
-__device__ __forceinline__ float2 resample_input(const StageView& a, unsigned long long phase_inc, long long g) {
+template <class View>
+__device__ __forceinline__ float2 resample_input(const View& a, unsigned long long phase_inc, long long g) {
   if (g < 0) return make_float2(0.0f, 0.0f);  // before startRecording: zero history
   float2 v = resample_raw(a, g);
   if (a.kind == 2) return v;
@@ -103,12 +138,15 @@ __device__ __forceinline__ float2 resample_input(const StageView& a, unsigned lo
   return v;
 }
 
-__global__ void __launch_bounds__(kResampleThreads) k_resample(const __grid_constant__ ResampleArgs a) {
+// Args: ResampleArgs, or RingArgs for stage 0 of a catch-up
+template <class Args>
+__global__ void __launch_bounds__(kResampleThreads) k_resample(const __grid_constant__ Args a) {
   extern __shared__ float2 tile[];
   const int tid = threadIdx.x;
-  const StageChan& c = a.ch[blockIdx.x % a.n_ch];
+  const int j = blockIdx.x % a.n_ch;
+  const StageChan& c = a.ch[j];
   const int cta = blockIdx.x / a.n_ch;
-  const StageView v = stage_view(a, c);
+  const auto v = stage_view(a, c, j);
   const long long mb = c.m0 + static_cast<long long>(cta) * a.per_cta;  // first output of this CTA
   const int count = min(a.per_cta, c.n_out - cta * a.per_cta);
   if (count <= 0) return;
@@ -156,14 +194,16 @@ constexpr int kPolyThreads = 128;
 constexpr int kPolyOut = kPolyThreads * kPolyR;   // outputs per CTA
 constexpr int kPolyTile = kPolyOut + kPolyQ - 1;  // samples of one phase a CTA needs
 
-__global__ void __launch_bounds__(kPolyThreads) k_decimate_poly(const __grid_constant__ ResampleArgs a, const float* __restrict__ taps_pq /* [D][kPolyQ]: h[q D + p], zero padded */) {
+template <class Args>
+__global__ void __launch_bounds__(kPolyThreads) k_decimate_poly(const __grid_constant__ Args a, const float* __restrict__ taps_pq /* [D][kPolyQ]: h[q D + p], zero padded */) {
   __shared__ float2 tile[2][kPolyTile];
   __shared__ float htap[2][kPolyQ];
   const int tid = threadIdx.x;
   const int D = a.decim;
-  const StageChan& c = a.ch[blockIdx.x % a.n_ch];
+  const int j = blockIdx.x % a.n_ch;
+  const StageChan& c = a.ch[j];
   const int cta = blockIdx.x / a.n_ch;
-  const StageView sv = stage_view(a, c);
+  const auto sv = stage_view(a, c, j);
   const long long mb = c.m0 + static_cast<long long>(cta) * kPolyOut;  // first output of this CTA
   const int count = min(kPolyOut, c.n_out - cta * kPolyOut);
   if (count <= 0) return;
