@@ -57,6 +57,26 @@ extern "C" {
                                        runs on a worker thread while push k+1 is in the kernels (the reference decouples the
                                        same two halves through its 1-slot mailbox, notification.h:14-26). Results are
                                        collected with b2s_band_sync; b2s_band_push must be given out = NULL. */
+/* Sub-frames: detect from every sample of a frame's stride instead of its first fft_size samples only (opt-in; off by default).
+ * Frame k has r = floor(frame_stride_samples / fft_size) sub-frames; sub-frame j is the fft_size samples starting at
+ * k * frame_stride_samples + j * fft_size (j = 0 ... r-1); samples past r * fft_size in a stride stay unused. Each sub-frame is
+ * windowed, transformed, shifted and squared exactly as a frame is without the flag, p_j[b] = |X_j[b]|^2 / fs, and the frame's
+ * linear power row is
+ *   MEAN: acc = p_0; acc = acc + p_j for j = 1 ... r-1 in that order (fp32, round to nearest); p = acc / (float)r (fp32 division)
+ *   MAX:  p = fmaxf over j = 0 ... r-1
+ * The dB row, the first maximum (peak_index / peak_value) and b2s_psd's power_lin are then computed from p as without the flag.
+ *   - Frames, their clock, event frames, b2s_band_record_from positions, the spectrogram schedule and an attached recorder bank's
+ *     input do not change. Noise learning, the Averager, the detector and the tracker see the new rows.
+ *   - With r = 1 (frame_stride_samples < 2 * fft_size) either flag changes nothing, bit for bit.
+ *   - Both flags together are refused (B2S_E_INVALID) by b2s_band_create and b2s_psd.
+ *   - Input: a push (or b2s_psd) of n_frames frames reads (n_frames - 1) * frame_stride_samples + r * fft_size samples, host or
+ *     device; with an attached recorder bank the rule stays n_frames * frame_stride_samples.
+ *   - A band snapshot records the flags; a load into a band whose two sub-frame bits differ is refused (the learned noise depends
+ *     on them).
+ * MEAN suits weak continuous signals: the mean of r periodograms has a smaller spread, so the learned noise maximum sits lower.
+ * MAX suits bursts shorter than a stride: the mean would dilute a burst that fills one sub-frame by 10 log10(r) dB. */
+#define B2S_FLAG_SUBFRAME_MEAN 0x400
+#define B2S_FLAG_SUBFRAME_MAX 0x800
 
 /* Construction-time parameters. The reference takes them from Config / Device / the setupChains lambdas
  * (sdr_device.cpp:148-167, transmission.h:17-25, config.h:24-38). */

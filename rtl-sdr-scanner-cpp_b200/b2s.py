@@ -22,6 +22,8 @@ MAX_TX = 64
 IQ_CS8, IQ_CF32 = 0, 1
 FLAG_IQ_ON_DEVICE = 0x100
 FLAG_ASYNC = 0x200
+FLAG_SUBFRAME_MEAN = 0x400  # a frame's PSD row is the mean of its stride's floor(stride / N) sub-frame periodograms (include/b2s.h)
+FLAG_SUBFRAME_MAX = 0x800   # ... or their per-bin maximum; make_config(flags=...) and Engine.psd pass them through
 
 
 class BandConfig(C.Structure):

@@ -177,27 +177,27 @@ int prepare_kernel(b2s_engine* e, K kernel, int threads, size_t smem, int* ctas_
 }
 
 // K1 launcher -------------------------------------------------------------------------------------------------
-template <int N, int MODE, bool LIN>
+template <int N, int MODE, bool LIN, bool SUB>
 int launch_spectrum_v(b2s_engine* e, const SpectralArgs& a, cudaStream_t stream) {
   using PL = FftPlanT<N>;
   constexpr int T = N / PL::E;
   const size_t smem = sizeof(float2) * (exchange_elems<N>() + TwiddleLayout<N>::SMEM) + (MODE == kModeCs8Tma ? 2 * N : 0);
   int ctas_per_sm = 1;
-  int rc = prepare_kernel(e, k_spectrum<N, MODE, LIN>, T, smem, &ctas_per_sm);
+  int rc = prepare_kernel(e, k_spectrum<N, MODE, LIN, SUB>, T, smem, &ctas_per_sm);
   if (rc) return rc;
   const int grid = std::min(a.n_frames, e->sm_count * ctas_per_sm);
-  k_spectrum<N, MODE, LIN><<<grid, T, smem, stream>>>(a);
+  k_spectrum<N, MODE, LIN, SUB><<<grid, T, smem, stream>>>(a);
   CU(cudaGetLastError());
   return 0;
 }
 // k_spectrum3: N = RA * 1024 directly (RA = 4, 8, 16), or N = S * 16384 through the split mode (S = a.split > 1)
-template <int RA, int MODE, bool LIN, int S>
+template <int RA, int MODE, bool LIN, int S, bool SUB>
 int launch_spectrum3_v(b2s_engine* e, const SpectralArgs& a, cudaStream_t stream) {
   constexpr int T = RA * 32;
   constexpr bool SPLIT = S > 1;
   const size_t smem = sizeof(float2) * (RA * kBlockPitch + 31 * 32) + (MODE == kModeCs8Tma ? (SPLIT ? 2 * kSplitStageBytes : 2 * RA * 1024) : 0);
   int ctas_per_sm = 1;
-  int rc = prepare_kernel(e, k_spectrum3<RA, MODE, LIN, S>, T, smem, &ctas_per_sm);
+  int rc = prepare_kernel(e, k_spectrum3<RA, MODE, LIN, S, SUB>, T, smem, &ctas_per_sm);
   if (rc) return rc;
   if (!a.work_counter) return fail(B2S_E_INVALID, "k_spectrum3 needs a work counter");
   const int items = a.n_frames * S;
@@ -207,7 +207,7 @@ int launch_spectrum3_v(b2s_engine* e, const SpectralArgs& a, cudaStream_t stream
     if (!a.peak_packed || !a.split_tw || !a.split_ws) return fail(B2S_E_INVALID, "split-mode tables are missing");
     CU(cudaMemsetAsync(a.peak_packed, 0, sizeof(unsigned long long) * a.n_frames, stream));
   }
-  k_spectrum3<RA, MODE, LIN, S><<<grid, T, smem, stream>>>(a);
+  k_spectrum3<RA, MODE, LIN, S, SUB><<<grid, T, smem, stream>>>(a);
   CU(cudaGetLastError());
   if (SPLIT) {
     k_peak_unpack<<<(a.n_frames + 255) / 256, 256, 0, stream>>>(a.peak_packed, a.n_frames, a.peak_index, a.peak_value);
@@ -226,19 +226,25 @@ constexpr bool k1_is_v3(int n) { return n >= 4096; }
 constexpr long long kMaxPushBins = 1LL << 30;
 constexpr int default_max_frames(int n) { return n > 16 * kSplitM ? static_cast<int>(kMaxPushBins / n) : 4096; }
 
-template <int N, int MODE>
-int launch_spectrum_t(b2s_engine* e, const SpectralArgs& a, cudaStream_t stream) {
+template <int N, int MODE, bool SUB>
+int launch_spectrum_s(b2s_engine* e, const SpectralArgs& a, cudaStream_t stream) {
   // the |X|^2/fs debug rows come from a debug twin of each instantiation (parity tests); the product one stays lean
   if constexpr (N > kSplitM) {
-    if (a.power_lin) return launch_spectrum3_v<16, MODE, true, N / kSplitM>(e, a, stream);
-    return launch_spectrum3_v<16, MODE, false, N / kSplitM>(e, a, stream);
+    if (a.power_lin) return launch_spectrum3_v<16, MODE, true, N / kSplitM, SUB>(e, a, stream);
+    return launch_spectrum3_v<16, MODE, false, N / kSplitM, SUB>(e, a, stream);
   } else if constexpr (k1_is_v3(N)) {
-    if (a.power_lin) return launch_spectrum3_v<N / 1024, MODE, true, 1>(e, a, stream);
-    return launch_spectrum3_v<N / 1024, MODE, false, 1>(e, a, stream);
+    if (a.power_lin) return launch_spectrum3_v<N / 1024, MODE, true, 1, SUB>(e, a, stream);
+    return launch_spectrum3_v<N / 1024, MODE, false, 1, SUB>(e, a, stream);
   } else {
-    if (a.power_lin) return launch_spectrum_v<N, MODE, true>(e, a, stream);
-    return launch_spectrum_v<N, MODE, false>(e, a, stream);
+    if (a.power_lin) return launch_spectrum_v<N, MODE, true, SUB>(e, a, stream);
+    return launch_spectrum_v<N, MODE, false, SUB>(e, a, stream);
   }
+}
+// a.sub_r > 1 (sub-frames) runs the SUB instantiations; r = 1 runs the kernels of a frame without sub-frames
+template <int N, int MODE>
+int launch_spectrum_t(b2s_engine* e, const SpectralArgs& a, cudaStream_t stream) {
+  if (a.sub_r > 1) return launch_spectrum_s<N, MODE, true>(e, a, stream);
+  return launch_spectrum_s<N, MODE, false>(e, a, stream);
 }
 
 template <int MODE>
@@ -288,13 +294,20 @@ void plan_radices(int n, int* r) {
   }
 }
 
+// Sub-frames a frame's PSD row is made of: floor(stride / N) with B2S_FLAG_SUBFRAME_MEAN or _MAX, else 1.
+constexpr int kSubframeFlags = B2S_FLAG_SUBFRAME_MEAN | B2S_FLAG_SUBFRAME_MAX;
+int subframes(const b2s_band_config& c) { return (c.flags & kSubframeFlags) ? c.frame_stride_samples / c.fft_size : 1; }
+
 struct SpectralTables {
   DevBuf<float> wscale;
   DevBuf<float2> twiddle, split_tw, split_ws;
   DevBuf<int> work_counter;  // k_spectrum3's {next item, finished CTAs}; the kernel leaves both at zero
   int split = 1;
+  int sub_r = 1, sub_max = 0;  // sub-frames per frame and their reduction (B2S_FLAG_SUBFRAME_*)
   int build(const b2s_band_config& cfg) {
     const int n = cfg.fft_size;
+    sub_r = subframes(cfg);
+    sub_max = (cfg.flags & B2S_FLAG_SUBFRAME_MAX) != 0;
     std::vector<float> w;
     make_window(cfg, w);
     if (cfg.iq_format == B2S_IQ_CS8) {
@@ -356,6 +369,8 @@ struct SpectralTables {
     sa.split = split;
     sa.split_tw = split_tw.p;
     sa.split_ws = split_ws.p;
+    sa.sub_r = sub_r;
+    sa.sub_max = sub_max;
   }
 };
 
@@ -367,6 +382,7 @@ int validate_config(const b2s_band_config& c) {
   if (c.sample_rate_hz <= 0) return fail(B2S_E_INVALID, "sample_rate_hz must be positive");
   if (c.frame_stride_samples < c.fft_size) return fail(B2S_E_INVALID, "frame_stride_samples (%d) < fft_size", c.frame_stride_samples);
   if (c.iq_format != B2S_IQ_CS8 && c.iq_format != B2S_IQ_CF32) return fail(B2S_E_INVALID, "unknown iq_format %d", c.iq_format);
+  if ((c.flags & kSubframeFlags) == kSubframeFlags) return fail(B2S_E_INVALID, "B2S_FLAG_SUBFRAME_MEAN and B2S_FLAG_SUBFRAME_MAX exclude each other");
   if (c.window_kind == B2S_WINDOW_USER && !c.window_taps) return fail(B2S_E_INVALID, "window_taps is NULL");
   if (c.grouping_x < 1 || c.grouping_x > 65) return fail(B2S_E_INVALID, "grouping_x must be in 1..65");
   if (c.grouping_y < 1 || c.grouping_y > 256) return fail(B2S_E_INVALID, "grouping_y must be in 1..256");
@@ -556,12 +572,13 @@ void put_band_config(StateWriter& w, b2s_band_config c) {
 void get_band_config(StateReader& r, b2s_band_config& c) {
   band_config_fields(c, [&](auto& v) { v = r.get<std::decay_t<decltype(v)>>(); });
 }
-// Two creation configs that a snapshot may move between: equal bit for bit except the centre and range (state), the flags and the
-// sizing fields.
+// Two creation configs that a snapshot may move between: equal bit for bit except the centre and range (state), the flags other
+// than the sub-frame bits (the learned noise depends on those) and the sizing fields.
 bool same_band_config(b2s_band_config a, b2s_band_config b) {
   StateWriter x, y;
   for (auto* c : {&a, &b}) {
-    c->center_hz = c->range_lo_hz = c->range_hi_hz = c->flags = c->max_frames_per_push = c->detect_capacity = 0;
+    c->center_hz = c->range_lo_hz = c->range_hi_hz = c->max_frames_per_push = c->detect_capacity = 0;
+    c->flags &= kSubframeFlags;
     c->window_taps = nullptr;
   }
   put_band_config(x, a);
@@ -1503,8 +1520,8 @@ static int band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms
   auto chunk_len = [&](size_t done) { return std::min(n_frames - done, pipe); };
   auto start_copy = [&](size_t done, int slot) -> int {
     const size_t chunk = chunk_len(done);
-    // the last frame needs N samples only, unless a bank reads the whole stream
-    const size_t bytes = b->bank ? chunk * stride_bytes : (chunk - 1) * stride_bytes + static_cast<size_t>(b->cfg.fft_size) * bytes_per_sample;
+    // the last frame needs its r sub-frames of N samples only (r = 1 without sub-frames), unless a bank reads the whole stream
+    const size_t bytes = b->bank ? chunk * stride_bytes : (chunk - 1) * stride_bytes + static_cast<size_t>(subframes(b->cfg)) * b->cfg.fft_size * bytes_per_sample;
     CU(cudaMemcpyAsync(b->d_iq[slot].p, static_cast<const char*>(iq) + done * stride_bytes, bytes, cudaMemcpyHostToDevice, b->copy_stream));
     CU(cudaEventRecord(b->copy_done[slot], b->copy_stream));
     b->prof.h2d_bytes += bytes;
@@ -1910,7 +1927,7 @@ int b2s_psd(b2s_engine* e, const b2s_band_config* cfg, const void* iq, size_t n_
   const size_t n = c.fft_size;
   const size_t bps = c.iq_format == B2S_IQ_CS8 ? 2 : 8;
   const size_t stride = static_cast<size_t>(c.frame_stride_samples) * bps;
-  const size_t bytes = (n_frames - 1) * stride + n * bps;
+  const size_t bytes = (n_frames - 1) * stride + static_cast<size_t>(subframes(c)) * n * bps;
   rc = tables.build(c);
   if (!rc) rc = diq.alloc(bytes);
   if (!rc) rc = dpsd.alloc(n_frames * n);

@@ -699,8 +699,8 @@ struct b2s_band : public DeviceQueries {
     get_band_config(r, saved);
     if (!r.ok) return bad("the config block is truncated");
     if (!same_band_config(saved, cfg))
-      return bad("the snapshot was made with another configuration (every field but center_hz, range_lo_hz, range_hi_hz, flags, max_frames_per_push and "
-                 "detect_capacity must match)");
+      return bad("the snapshot was made with another configuration (every field but center_hz, range_lo_hz, range_hi_hz, the flags other than "
+                 "B2S_FLAG_SUBFRAME_*, max_frames_per_push and detect_capacity must match)");
     if (cfg.window_kind == B2S_WINDOW_USER) {
       const uint8_t* taps = r.span(sizeof(float) * n);
       if (!taps) return bad("the config block is truncated");

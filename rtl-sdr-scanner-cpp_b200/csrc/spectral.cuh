@@ -179,7 +179,20 @@ struct SpectralArgs {
   const float2* split_tw;       // [S][16384]  W_N^(n' c)
   const float2* split_ws;       // [S]         W_S^j
   unsigned long long* peak_packed;  // [n_frames], zeroed before the launch: max over the S classes of (ordered(value) << 32 | ~index)
+  // ---- sub-frames (the SUB instantiations only, B2S_FLAG_SUBFRAME_*) ----
+  int sub_r;                    // sub-frames per frame, r >= 2: sub-frame j starts at iq + k * frame_stride_bytes + j * N samples
+  int sub_max;                  // reduction over the sub-frames' |X|^2/fs: 0 = mean (sum in order, then / r), 1 = maximum
 };
+
+// One sub-frame's |X|^2/fs folded into the frame's partial: MEAN adds in sub-frame order, MAX keeps the larger. On the last
+// sub-frame the caller divides the mean by r.
+__device__ __forceinline__ float sub_fold(float part, float pw, int sub, int sub_max) {
+  if (sub == 0) return pw;
+  return sub_max ? fmaxf(part, pw) : __fadd_rn(part, pw);
+}
+__device__ __forceinline__ float sub_finish(float acc, const SpectralArgs& a) {
+  return a.sub_max ? acc : __fdiv_rn(acc, static_cast<float>(a.sub_r));
+}
 
 // tw points at this pass's [m-1][k] table (shared or global)
 template <int N, int R, int P, int E, int T>
@@ -240,7 +253,10 @@ __device__ __forceinline__ float fast_log2(float x) {
   return y;
 }
 
-template <int N, int MODE, bool DEBUG_LIN>
+// SUB (B2S_FLAG_SUBFRAME_*): a frame is a_.sub_r sub-frames of N samples, transformed one after the other by the CTA that takes
+// the frame; the TMA buffer is filled with the next sub-frame (or the next frame's first) behind each pass 0. The thread that owns
+// bin b in the epilogue folds every sub-frame's |X|^2/fs into acc[] (registers) and the last sub-frame converts the reduced row.
+template <int N, int MODE, bool DEBUG_LIN, bool SUB>
 __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralArgs a) {
   using PL = FftPlanT<N>;
   using TL = TwiddleLayout<N>;
@@ -262,6 +278,12 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
   const int tid = threadIdx.x;
   const int lane = tid & 31, warp = tid >> 5;
   const char* base = static_cast<const char*>(a.iq);
+  // first sample of sub-frame `sub` of `frame` (sub = 0 without SUB)
+  auto src = [&](long long frame, int sub) {
+    const char* p = base + frame * a.frame_stride_bytes;
+    if (SUB) p += static_cast<long long>(sub) * N * (MODE == kModeCf32 ? 8 : 2);
+    return p;
+  };
 
   if (MODE == kModeCs8Tma) {
     if (tid == 0) {
@@ -286,13 +308,15 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
   if (MODE == kModeCs8Tma) {
     if (tid == 0 && static_cast<int>(blockIdx.x) < a.n_frames) {
       mbar_arrive_expect_tx(&full_bar, 2 * N);
-      bulk_g2s(raw, base + static_cast<long long>(blockIdx.x) * a.frame_stride_bytes, 2 * N, &full_bar);
+      bulk_g2s(raw, src(blockIdx.x, 0), 2 * N, &full_bar);
     }
   }
 
   uint32_t parity = 0;
   for (int frame = blockIdx.x; frame < a.n_frames; frame += gridDim.x) {
     float2 v[E];
+    float acc[SUB ? E : 1];  // SUB: the frame's partial reduction of the bins this thread owns in the epilogue
+    for (int sub = 0; sub < (SUB ? a.sub_r : 1); ++sub) {
     // ---------------- pass 0: unpack + window, radix R0, no twiddles (P = 1) ----------------
     {
       constexpr int NB = N / R0, BPT = E / R0;
@@ -309,10 +333,10 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
             const char2 s = reinterpret_cast<const char2*>(raw)[n];
             v[u * R0 + m] = make_float2(static_cast<float>(s.x) * w, static_cast<float>(s.y) * w);
           } else if (MODE == kModeCs8Direct) {
-            const signed char* fp = reinterpret_cast<const signed char*>(base + static_cast<long long>(frame) * a.frame_stride_bytes);
+            const signed char* fp = reinterpret_cast<const signed char*>(src(frame, sub));
             v[u * R0 + m] = make_float2(static_cast<float>(fp[2 * n]) * w, static_cast<float>(fp[2 * n + 1]) * w);
           } else {
-            const float* fp = reinterpret_cast<const float*>(base + static_cast<long long>(frame) * a.frame_stride_bytes);
+            const float* fp = reinterpret_cast<const float*>(src(frame, sub));
             v[u * R0 + m] = make_float2(fp[2 * n] * w, fp[2 * n + 1] * w);
           }
         }
@@ -321,12 +345,17 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
       pass_store<N, R0, 1, E, T>(X, v, tid);
     }
     __syncthreads();
-    // the staging buffer is consumed: start the copy of this CTA's next frame (overlaps the remaining passes)
+    // the staging buffer is consumed: start the copy of this CTA's next (sub-)frame (overlaps the remaining passes)
     if (MODE == kModeCs8Tma && tid == 0) {
-      const int next = frame + gridDim.x;
-      if (next < a.n_frames) {
+      if (SUB && sub + 1 < a.sub_r) {
         mbar_arrive_expect_tx(&full_bar, 2 * N);
-        bulk_g2s(raw, base + static_cast<long long>(next) * a.frame_stride_bytes, 2 * N, &full_bar);
+        bulk_g2s(raw, src(frame, sub + 1), 2 * N, &full_bar);
+      } else {
+        const int next = frame + gridDim.x;
+        if (next < a.n_frames) {
+          mbar_arrive_expect_tx(&full_bar, 2 * N);
+          bulk_g2s(raw, src(next, 0), 2 * N, &full_bar);
+        }
       }
     }
     // ---------------- middle passes ----------------
@@ -348,6 +377,12 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
     pass_load<N, RL, E, T>(X, v, tid);
     constexpr int PL_ = (NP == 4) ? P3 : (NP == 3 ? P2 : P1);
     pass_twiddle_butterfly<N, RL, PL_, E, T>(v, NP == 4 ? tw3 : (NP == 3 ? tw2 : tw1), tid);
+    if (SUB) {
+#pragma unroll
+      for (int i = 0; i < E; ++i) acc[i] = sub_fold(acc[i], fmaf(v[i].x, v[i].x, v[i].y * v[i].y) * a.inv_fs, sub, a.sub_max);
+      if (sub + 1 < a.sub_r) __syncthreads();  // every thread has read X before the next sub-frame's pass 0 overwrites it
+    }
+    }
 
     // thread holds bins k = b + m * (N / RL): |X|^2 / fs -> 10 log10 (psd.cpp:18), written at (k + N/2) mod N
     float* row = a.psd_db + static_cast<size_t>(frame) * N;
@@ -362,7 +397,7 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
         for (int m = 0; m < RL; ++m) {
           const float2 z = v[u * RL + m];
           const int j = (b + m * NB + N / 2) & (N - 1);
-          const float pw = fmaf(z.x, z.x, z.y * z.y) * a.inv_fs;
+          const float pw = SUB ? sub_finish(acc[u * RL + m], a) : fmaf(z.x, z.x, z.y * z.y) * a.inv_fs;
           const float db = kDbPerLog2 * fast_log2(pw);
           row[j] = db;
           if (DEBUG_LIN) a.power_lin[static_cast<size_t>(frame) * N + j] = pw;
