@@ -434,159 +434,9 @@ static float least_sum_reaching(float level, int divisor) {
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// snapshots of a band or a recorder bank (b2s_*_save_state / b2s_*_load_state; the format is described in DESIGN.md §3)
-//   header   u32 magic "B2ST", u32 version, u32 kind, u64 total length
-//   sections u32 tag, u64 payload length, payload; in a fixed order per kind, the config block first
-//   trailer  u64 FNV-1a of every byte before it
-// Every value is written field by field in the host's (little-endian) byte order, so a snapshot holds no padding.
+// snapshots of a band or a recorder bank: the format
 // ------------------------------------------------------------------------------------------------------------
-static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "snapshots are defined as little-endian");
-namespace {
-
-constexpr uint32_t kStateMagic = 0x54533242u;  // "B2ST"
-constexpr uint32_t kStateVersion = 1;
-constexpr uint32_t kStateBand = 1, kStateBank = 2;
-constexpr size_t kStateHeader = 20;
-constexpr uint32_t state_tag(const char (&s)[5]) {
-  return static_cast<uint32_t>(s[0]) | static_cast<uint32_t>(s[1]) << 8 | static_cast<uint32_t>(s[2]) << 16 | static_cast<uint32_t>(s[3]) << 24;
-}
-
-uint64_t fnv1a64(const uint8_t* p, size_t n) {
-  uint64_t h = 0xcbf29ce484222325ull;
-  for (size_t i = 0; i < n; ++i) h = (h ^ p[i]) * 0x100000001b3ull;
-  return h;
-}
-
-struct StateWriter {
-  std::vector<uint8_t> out;
-  size_t section_at = 0;
-  template <typename T>
-  void put(T v) {
-    static_assert(std::is_arithmetic<T>::value, "fields are written one by one");
-    bytes(&v, sizeof(T));
-  }
-  void bytes(const void* p, size_t n) { out.insert(out.end(), static_cast<const uint8_t*>(p), static_cast<const uint8_t*>(p) + n); }
-  uint8_t* grow(size_t n) {  // n zeroed bytes to be filled in place (by a device-to-host copy)
-    out.resize(out.size() + n);
-    return out.data() + out.size() - n;
-  }
-  void begin(uint32_t kind) {
-    put(kStateMagic);
-    put(kStateVersion);
-    put(kind);
-    put<uint64_t>(0);
-  }
-  void open(uint32_t tag) {
-    put(tag);
-    section_at = out.size();
-    put<uint64_t>(0);
-  }
-  void close() {
-    const uint64_t len = out.size() - section_at - sizeof(uint64_t);
-    std::memcpy(out.data() + section_at, &len, sizeof(len));
-  }
-  void finish() {
-    const uint64_t total = out.size() + sizeof(uint64_t);
-    std::memcpy(out.data() + 12, &total, sizeof(total));
-    put(fnv1a64(out.data(), out.size()));
-  }
-};
-
-// Bounds-checked reads: a read past the current section clears `ok` and reads zeros.
-struct StateReader {
-  const uint8_t* p = nullptr;
-  size_t end = 0, at = 0, section_end = 0;
-  bool ok = true;
-  const uint8_t* span(size_t n) {
-    if (!ok || n > section_end - at) {
-      ok = false;
-      return nullptr;
-    }
-    at += n;
-    return p + at - n;
-  }
-  template <typename T>
-  T get() {
-    T v{};
-    if (const uint8_t* s = span(sizeof(T))) std::memcpy(&v, s, sizeof(T));
-    return v;
-  }
-  bool flag() {
-    const uint8_t v = get<uint8_t>();
-    ok = ok && v <= 1;
-    return v != 0;
-  }
-  // the next section, which must have this tag and lie within the snapshot
-  bool open(uint32_t tag) {
-    if (!ok) return false;
-    section_end = end;
-    const uint32_t t = get<uint32_t>();
-    const uint64_t len = get<uint64_t>();
-    if (!ok || t != tag || len > end - at) return ok = false;
-    section_end = at + len;
-    return true;
-  }
-  // the section was read to its last byte
-  bool close() { return ok = ok && at == section_end; }
-  // `count` items of `item` bytes fit in the rest of the section
-  bool fits(uint64_t count, size_t item) { return ok = ok && count <= (section_end - at) / item; }
-};
-
-// header and checksum of a snapshot of `kind`; on success `r` is positioned at the first section
-int open_state(const void* buf, size_t len, uint32_t kind, StateReader& r, const char* who) {
-  const uint8_t* p = static_cast<const uint8_t*>(buf);
-  if (len < kStateHeader + sizeof(uint64_t)) return fail(B2S_E_INVALID, "%s: %zu bytes are too short for a snapshot", who, len);
-  uint32_t magic, version, k;
-  uint64_t total, sum;
-  std::memcpy(&magic, p, 4);
-  std::memcpy(&version, p + 4, 4);
-  std::memcpy(&k, p + 8, 4);
-  std::memcpy(&total, p + 12, 8);
-  std::memcpy(&sum, p + len - 8, 8);
-  if (magic != kStateMagic) return fail(B2S_E_INVALID, "%s: not a b2s snapshot (magic %08x)", who, magic);
-  if (version != kStateVersion) return fail(B2S_E_INVALID, "%s: snapshot format version %u, this library reads version %u", who, version, kStateVersion);
-  if (k != kind) return fail(B2S_E_INVALID, "%s: the snapshot is of a %s, not of a %s", who, k == kStateBand ? "band" : k == kStateBank ? "recorder bank" : "unknown kind",
-                             kind == kStateBand ? "band" : "recorder bank");
-  if (total != len) return fail(B2S_E_INVALID, "%s: the snapshot is %llu bytes long, %zu were given", who, static_cast<unsigned long long>(total), len);
-  if (fnv1a64(p, len - 8) != sum) return fail(B2S_E_INVALID, "%s: checksum mismatch (the snapshot is damaged)", who);
-  r = StateReader{};
-  r.p = p;
-  r.end = r.section_end = len - 8;
-  r.at = kStateHeader;
-  return 0;
-}
-
-// every field of b2s_band_config except the window_taps pointer, in declaration order
-template <typename F>
-void band_config_fields(b2s_band_config& c, F&& f) {
-  f(c.fft_size), f(c.sample_rate_hz), f(c.frame_stride_samples), f(c.iq_format), f(c.iq_scale), f(c.window_kind), f(c.grouping_x), f(c.grouping_y);
-  f(c.group_size_bins), f(c.start_level), f(c.stop_level), f(c.learn_frames), f(c.center_hz), f(c.range_lo_hz), f(c.range_hi_hz), f(c.n_ignored);
-  for (auto& v : c.ignored_lo_hz) f(v);
-  for (auto& v : c.ignored_hi_hz) f(v);
-  f(c.tuning_step_hz), f(c.min_time_ms), f(c.timeout_ms), f(c.max_time_ms), f(c.spectrogram_out_size), f(c.spectrogram_interval_ms), f(c.flags);
-  f(c.max_frames_per_push), f(c.detect_capacity), f(c.noise_learning_ms);
-}
-void put_band_config(StateWriter& w, b2s_band_config c) {
-  band_config_fields(c, [&](auto& v) { w.put(v); });
-}
-void get_band_config(StateReader& r, b2s_band_config& c) {
-  band_config_fields(c, [&](auto& v) { v = r.get<std::decay_t<decltype(v)>>(); });
-}
-// Two creation configs that a snapshot may move between: equal bit for bit except the centre and range (state), the flags other
-// than the sub-frame bits (the learned noise depends on those) and the sizing fields.
-bool same_band_config(b2s_band_config a, b2s_band_config b) {
-  StateWriter x, y;
-  for (auto* c : {&a, &b}) {
-    c->center_hz = c->range_lo_hz = c->range_hi_hz = c->max_frames_per_push = c->detect_capacity = 0;
-    c->flags &= kSubframeFlags;
-    c->window_taps = nullptr;
-  }
-  put_band_config(x, a);
-  put_band_config(y, b);
-  return x.out == y.out;
-}
-
-}  // namespace
+#include "snapshot.h"
 
 // ------------------------------------------------------------------------------------------------------------
 // band
@@ -1162,111 +1012,41 @@ int band_auto_decide(b2s_band* b) {
   return bank_catch_up(k, std::move(catch_up));
 }
 
-// ---- recorder bank snapshot: the raw-sample carry, then per channel its position, its rows of the stages' carries and its chunks ----
-void put_bank_config(StateWriter& w, const b2s_recorder_bank* k) {
-  w.put<int32_t>(k->sample_rate);
-  w.put<int32_t>(k->bandwidth);
-  w.put<int32_t>(k->iq_format);
-  w.put<float>(k->iq_scale);
-  w.put<int32_t>(k->n_ch);
-}
-// the carry of channel c in stage si >= 1: the first hc samples of its row
-size_t stage_carry_bytes(const b2s_recorder_bank::Stage& st) { return sizeof(float2) * st.hc; }
-
-int bank_save(b2s_recorder_bank* k, std::vector<uint8_t>& out) {
+// ---- recorder bank snapshot (snapshot.h) ----
+// channel i's row of stage si >= 1, whose first hc samples are its carry
+float2* stage_row(b2s_recorder_bank* k, size_t si, int i) { return k->stages[si].buf.p + k->stages[si].stride * i; }
+// Finishes the bank's work, then describes it: its config and sizes, and for a save its device arrays
+int bank_image(b2s_recorder_bank* k, snapshot::BankImage& s) {
   int rc = bank_settle(k);
   if (rc) return rc;
   CU(cudaSetDevice(k->engine->device));
   CU(cudaStreamSynchronize(k->stream));
-  StateWriter w;
-  w.begin(kStateBank);
-  w.open(state_tag("CONF"));
-  put_bank_config(w, k);
-  w.close();
-  w.open(state_tag("RAWC"));
-  const size_t raw = static_cast<size_t>(k->stages[0].hc) * k->raw_bytes();
-  CU(cudaMemcpy(w.grow(raw), k->carry_raw.p, raw, cudaMemcpyDeviceToHost));
-  w.close();
-  const size_t chunk_bytes = 2 * static_cast<size_t>(k->chunk_samples);
-  for (int i = 0; i < k->n_ch; ++i) {
-    const auto& c = k->ch[i];
-    w.open(state_tag("CHAN"));
-    w.put<uint8_t>(c.recording);
-    w.put<uint8_t>(c.timed);
-    w.put<uint64_t>(c.phase_inc);
-    w.put<int64_t>(c.seen);
-    w.put<int64_t>(c.start_ms);
-    w.put<int64_t>(c.flushed);
-    for (size_t si = 1; si < k->stages.size(); ++si) {
-      const auto& st = k->stages[si];
-      CU(cudaMemcpy(w.grow(stage_carry_bytes(st)), st.buf.p + st.stride * i, stage_carry_bytes(st), cudaMemcpyDeviceToHost));
-    }
-    w.put<uint64_t>(c.chunks.size());
-    for (const auto& chunk : c.chunks) w.bytes(chunk.data(), chunk_bytes);
-    w.put<uint64_t>(c.tail.size());
-    w.bytes(c.tail.data(), c.tail.size());
-    w.close();
-  }
-  w.finish();
-  out.swap(w.out);
+  s.sample_rate = k->sample_rate, s.bandwidth = k->bandwidth, s.iq_format = k->iq_format, s.iq_scale = k->iq_scale, s.channels = k->n_ch;
+  s.raw_bytes = static_cast<size_t>(k->stages[0].hc) * k->raw_bytes();
+  s.chunk_bytes = 2 * static_cast<size_t>(k->chunk_samples);
+  for (size_t si = 1; si < k->stages.size(); ++si) s.carry_bytes.push_back(sizeof(float2) * k->stages[si].hc);
+  s.raw = k->carry_raw.p;
+  for (int i = 0; i < k->n_ch; ++i)
+    for (size_t si = 1; si < k->stages.size(); ++si) s.carry.push_back(stage_row(k, si, i));
   return 0;
 }
 
+int bank_save(b2s_recorder_bank* k, std::vector<uint8_t>& out) {
+  snapshot::BankImage s;
+  const int rc = bank_image(k, s);
+  return rc ? rc : snapshot::write(snapshot::kBank, k->stream, out, [&](snapshot::Writer& w) { snapshot::bank_sections(w, s, k->ch); });
+}
+
 int bank_load(b2s_recorder_bank* k, const void* buf, size_t len) {
-  const char* who = "b2s_recorder_bank_load_state";
-  int rc = bank_settle(k);
-  if (rc) return rc;
-  CU(cudaSetDevice(k->engine->device));
-  CU(cudaStreamSynchronize(k->stream));
-  StateReader r;
-  if ((rc = open_state(buf, len, kStateBank, r, who))) return rc;
-  auto bad = [&](const char* what) { return fail(B2S_E_INVALID, "%s: %s", who, what); };
-  if (!r.open(state_tag("CONF"))) return bad("the config block is missing or truncated");
-  {
-    StateWriter own;
-    put_bank_config(own, k);
-    const uint8_t* saved = r.span(own.out.size());
-    if (!saved || !r.close()) return bad("the config block has the wrong length");
-    if (std::memcmp(saved, own.out.data(), own.out.size()) != 0)
-      return bad("the snapshot was made by a bank with another sample rate, bandwidth, iq_format, iq_scale or channel count");
-  }
-  const size_t raw = static_cast<size_t>(k->stages[0].hc) * k->raw_bytes();
-  if (!r.open(state_tag("RAWC"))) return bad("the raw carry is missing or truncated");
-  const uint8_t* s_raw = r.span(raw);
-  if (!r.close()) return bad("the raw carry has the wrong length");
-  const size_t chunk_bytes = 2 * static_cast<size_t>(k->chunk_samples);
+  snapshot::BankImage s;
   std::vector<b2s_recorder_bank::Channel> s_ch(k->n_ch);
-  std::vector<std::vector<const uint8_t*>> s_carry(k->n_ch);
-  for (int i = 0; i < k->n_ch; ++i) {
-    auto& c = s_ch[i];
-    if (!r.open(state_tag("CHAN"))) return bad("a channel section is missing or truncated");
-    c.recording = r.flag();
-    c.timed = r.flag();
-    c.phase_inc = r.get<uint64_t>();
-    c.seen = r.get<int64_t>();
-    c.start_ms = r.get<int64_t>();
-    c.flushed = r.get<int64_t>();
-    for (size_t si = 1; si < k->stages.size(); ++si) s_carry[i].push_back(r.span(stage_carry_bytes(k->stages[si])));
-    const uint64_t n_chunks = r.get<uint64_t>();
-    if (!r.fits(n_chunks, chunk_bytes)) return bad("a channel's chunks are truncated");
-    for (uint64_t j = 0; j < n_chunks; ++j) {
-      const int8_t* src = reinterpret_cast<const int8_t*>(r.span(chunk_bytes));
-      c.chunks.emplace_back(src, src + chunk_bytes);
-    }
-    const uint64_t tail = r.get<uint64_t>();
-    if (!r.ok || tail >= chunk_bytes || tail % 2 != 0) return bad("a channel's incomplete chunk is malformed");
-    const int8_t* src = reinterpret_cast<const int8_t*>(r.span(tail));
-    if (tail > 0 && src) c.tail.assign(src, src + tail);
-    if (!r.close() || c.seen < 0 || c.flushed < 0) return bad("a channel section is malformed");
-  }
-  if (r.at != r.end) return bad("unexpected bytes after the last section");
-  CU(cudaMemcpyAsync(k->carry_raw.p, s_raw, raw, cudaMemcpyHostToDevice, k->stream));
-  for (int i = 0; i < k->n_ch; ++i) {
-    for (size_t si = 1; si < k->stages.size(); ++si) {
-      const auto& st = k->stages[si];
-      CU(cudaMemcpyAsync(st.buf.p + st.stride * i, s_carry[i][si - 1], stage_carry_bytes(st), cudaMemcpyHostToDevice, k->stream));
-    }
-  }
+  int rc = bank_image(k, s);
+  if (rc || (rc = snapshot::read(buf, len, snapshot::kBank, "b2s_recorder_bank_load_state", [&](snapshot::Reader& r) { snapshot::bank_sections(r, s, s_ch); })))
+    return rc;
+  CU(cudaMemcpyAsync(k->carry_raw.p, s.raw, s.raw_bytes, cudaMemcpyHostToDevice, k->stream));
+  size_t j = 0;
+  for (int i = 0; i < k->n_ch; ++i)
+    for (size_t si = 1; si < k->stages.size(); ++si, ++j) CU(cudaMemcpyAsync(stage_row(k, si, i), s.carry[j], s.carry_bytes[si - 1], cudaMemcpyHostToDevice, k->stream));
   CU(cudaStreamSynchronize(k->stream));
   k->ch.swap(s_ch);
   k->hist_end = 0;  // the history, which a snapshot does not hold, is of another stream
@@ -1745,14 +1525,7 @@ int b2s_band_load_state(b2s_band* b, const void* buf, size_t len) {
   if (!b || !buf) return fail(B2S_E_INVALID, "b2s_band_load_state: NULL argument");
   std::lock_guard<std::mutex> lock(b->mutex);
   CU(cudaSetDevice(b->engine->device));
-  const int rc = b->load_state(buf, len);
-  if (!rc) {  // the frames pushed before belong to another stream
-    b->hist_pieces.clear();
-    b->autorec = b2s_band::AutoRecord{};
-    std::lock_guard<std::mutex> lk(b->qmutex);
-    b->start_of.clear();
-  }
-  return rc;
+  return b->load_state(buf, len);
 }
 
 int b2s_band_record_from(b2s_band* b, int channel, int32_t shift_hz, int64_t frame) {

@@ -590,12 +590,8 @@ struct b2s_band : public DeviceQueries {
     return 0;
   }
 
-  // ---- snapshot (b2s_band_save_state / b2s_band_load_state): everything the next push reads and everything not yet collected ----
-  int download(void* dst, const void* src, size_t bytes) {
-    CU(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, stream));
-    CU(cudaStreamSynchronize(stream));  // `dst` lies in a vector that the next section may move
-    return 0;
-  }
+  // ---- snapshot (b2s_band_save_state / b2s_band_load_state; the format is snapshot.h's): everything the next push reads and everything
+  // not yet collected ----
   // the per-frame entry capacity of the next push (grow_capacity applies a pending growth first)
   int next_capacity() const { return std::min(cfg.fft_size, std::max(slot_capacity, wanted_capacity)); }
 
@@ -604,269 +600,81 @@ struct b2s_band : public DeviceQueries {
     if (rc) return rc;
     CU(cudaStreamSynchronize(stream));
     CU(cudaStreamSynchronize(track_stream));
-    const size_t n = cfg.fft_size, Y = cfg.grouping_y, M = std::max(cfg.spectrogram_out_size, 0);
-    StateWriter w;
-    w.begin(kStateBand);
-    w.open(state_tag("CONF"));
-    put_band_config(w, cfg);
-    w.bytes(user_window.data(), sizeof(float) * user_window.size());
-    w.close();
-    w.open(state_tag("SCAL"));
-    w.put<int32_t>(center);
-    w.put<int32_t>(tracker.p.range_lo);
-    w.put<int32_t>(tracker.p.range_hi);
-    w.put<int64_t>(frames_pushed);
-    w.put<uint8_t>(event_log);
-    w.put<int32_t>(stat_entries);
-    w.put<int32_t>(stat_rows);
-    w.put<int32_t>(next_capacity());
-    w.close();
-    w.open(state_tag("NOIS"));
-    w.put<uint32_t>(static_cast<uint32_t>(noise.size()));
-    for (auto& kv : noise) {
-      NoiseSlot& s = kv.second;
-      w.put<int32_t>(kv.first);
-      w.put<int32_t>(s.samples);
-      w.put<uint8_t>(s.ready);
-      w.put<uint8_t>(s.started);
-      w.put<int64_t>(s.start_ms);
-      if ((rc = download(w.grow(sizeof(float) * n), s.now(), sizeof(float) * n))) return rc;
-    }
-    w.close();
-    w.open(state_tag("SPEC"));
-    w.put<uint32_t>(static_cast<uint32_t>(spectro.size()));
-    for (auto& kv : spectro) {
-      w.put<int32_t>(kv.first);
-      w.put<int32_t>(kv.second.counter);
-      w.put<int64_t>(kv.second.last_send);
-      if ((rc = download(w.grow(sizeof(float) * M), kv.second.sum.p, sizeof(float) * M))) return rc;
-    }
-    w.close();
-    w.open(state_tag("AVGR"));
-    w.put<int32_t>(avg_frames);
-    if ((rc = download(w.grow(sizeof(float) * n), d_sum[sum_cur].p, sizeof(float) * n))) return rc;
-    if ((rc = download(w.grow(sizeof(float) * n), d_avg_last.p, sizeof(float) * n))) return rc;
-    if ((rc = download(w.grow(sizeof(float) * n * Y), d_ring[ring_cur].p, sizeof(float) * n * Y))) return rc;
-    w.close();
-    w.open(state_tag("SMAP"));
-    HostMap h;
-    if ((rc = download_state(h))) return rc;
-    w.put<int32_t>(static_cast<int32_t>(h.key.size()));
-    w.bytes(h.key.data(), sizeof(int) * h.key.size());
-    w.bytes(h.first.data(), sizeof(long long) * h.first.size());
-    w.bytes(h.last.data(), sizeof(long long) * h.last.size());
-    w.bytes(h.power.data(), sizeof(float) * h.power.size());
-    w.close();
+    snapshot::BandImage s;
+    s.center = center, s.range_lo = tracker.p.range_lo, s.range_hi = tracker.p.range_hi, s.frames_pushed = frames_pushed;
+    s.event_log = event_log, s.stat_entries = stat_entries, s.stat_rows = stat_rows, s.capacity = next_capacity();
+    for (auto& kv : noise) s.noise.push_back({kv.first, kv.second.samples, kv.second.ready, kv.second.started, kv.second.start_ms, kv.second.now()});
+    for (auto& kv : spectro) s.spectro.push_back({kv.first, kv.second.counter, kv.second.last_send, kv.second.sum.p});
+    s.avg_frames = avg_frames, s.avg_sum = d_sum[sum_cur].p, s.avg_last = d_avg_last.p, s.ring = d_ring[ring_cur].p;
+    CU(cudaMemcpy(&s.live, d_map_n.p, sizeof(int), cudaMemcpyDeviceToHost));
+    s.key = d_map_key.p, s.first = d_map_first.p, s.last = d_map_last.p, s.power = d_map_power.p;
     std::lock_guard<std::mutex> lk(qmutex);
-    w.open(state_tag("MBOX"));
-    w.put<uint32_t>(static_cast<uint32_t>(mailbox.size()));
-    for (const b2s_transmission& t : mailbox) {
-      w.put(t.shift_hz), w.put(t.flush), w.put(t.key), w.put(t.power);
-    }
-    w.close();
-    w.open(state_tag("EVNT"));
-    w.put<uint64_t>(events.size());
-    for (const b2s_signal_event& e : events) {
-      w.put(e.kind), w.put(e.key), w.put(e.shift_hz), w.put(e.reserved), w.put(e.frame), w.put(e.time_ms), w.put(e.first_ms), w.put(e.last_ms);
-    }
-    w.close();
-    w.open(state_tag("ROWS"));
-    w.put<uint64_t>(sent.size());
-    for (const SentRow& s : sent) {
-      w.put<int64_t>(s.time);
-      w.put<int32_t>(s.center);
-      w.bytes(s.row.data(), M);
-    }
-    w.close();
-    w.finish();
-    out.swap(w.out);
-    return 0;
+    return snapshot::write(snapshot::kBand, stream, out,
+                           [&](snapshot::Writer& w) { snapshot::band_sections(w, s, mailbox, events, sent, cfg, user_window.data()); });
   }
 
   int load_state(const void* buf, size_t len) {
-    const char* who = "b2s_band_load_state";
     int rc = drain();
     if (rc) return rc;
     CU(cudaStreamSynchronize(stream));
     CU(cudaStreamSynchronize(track_stream));
-    StateReader r;
-    if ((rc = open_state(buf, len, kStateBand, r, who))) return rc;
-    const int n = cfg.fft_size, Y = cfg.grouping_y, M = std::max(cfg.spectrogram_out_size, 0);
-    auto bad = [&](const char* what) { return fail(B2S_E_INVALID, "%s: %s", who, what); };
     // ---- read and check everything before anything changes ----
-    if (!r.open(state_tag("CONF"))) return bad("the config block is missing or truncated");
-    b2s_band_config saved{};
-    get_band_config(r, saved);
-    if (!r.ok) return bad("the config block is truncated");
-    if (!same_band_config(saved, cfg))
-      return bad("the snapshot was made with another configuration (every field but center_hz, range_lo_hz, range_hi_hz, the flags other than "
-                 "B2S_FLAG_SUBFRAME_*, max_frames_per_push and detect_capacity must match)");
-    if (cfg.window_kind == B2S_WINDOW_USER) {
-      const uint8_t* taps = r.span(sizeof(float) * n);
-      if (!taps) return bad("the config block is truncated");
-      if (std::memcmp(taps, user_window.data(), sizeof(float) * n) != 0) return bad("the snapshot was made with other user window taps");
-    }
-    if (!r.close()) return bad("the config block has the wrong length");
-
-    if (!r.open(state_tag("SCAL"))) return bad("the scalar section is missing or truncated");
-    const int32_t s_center = r.get<int32_t>(), s_lo = r.get<int32_t>(), s_hi = r.get<int32_t>();
-    const int64_t s_frames = r.get<int64_t>();
-    const bool s_log = r.flag();
-    const int32_t s_entries = r.get<int32_t>(), s_rows = r.get<int32_t>(), s_cap = r.get<int32_t>();
-    if (!r.close() || s_frames < 0 || s_entries < 0 || s_rows < 0 || s_cap < 1 || s_cap > n) return bad("the scalar section is malformed");
-
-    struct SavedNoise {
-      int32_t center, samples;
-      bool ready, started;
-      int64_t start_ms;
-      const uint8_t* thr;
-    };
-    std::vector<SavedNoise> s_noise;
-    if (!r.open(state_tag("NOIS"))) return bad("the noise section is missing or truncated");
-    const uint32_t n_noise = r.get<uint32_t>();
-    if (!r.fits(n_noise, 18 + sizeof(float) * n)) return bad("the noise section is truncated");
-    for (uint32_t i = 0; i < n_noise; ++i) {
-      SavedNoise s;
-      s.center = r.get<int32_t>();
-      s.samples = r.get<int32_t>();
-      s.ready = r.flag();
-      s.started = r.flag();
-      s.start_ms = r.get<int64_t>();
-      s.thr = r.span(sizeof(float) * n);
-      if (!r.ok || s.samples < 0 || (i > 0 && s.center <= s_noise.back().center)) return bad("the noise section is malformed");
-      s_noise.push_back(s);
-    }
-    if (!r.close()) return bad("the noise section has the wrong length");
-
-    struct SavedSpectro {
-      int32_t center, counter;
-      int64_t last_send;
-      const uint8_t* sum;
-    };
-    std::vector<SavedSpectro> s_spectro;
-    if (!r.open(state_tag("SPEC"))) return bad("the spectrogram section is missing or truncated");
-    const uint32_t n_spectro = r.get<uint32_t>();
-    if (!r.fits(n_spectro, 16 + sizeof(float) * M) || (M == 0 && n_spectro > 0)) return bad("the spectrogram section is malformed");
-    for (uint32_t i = 0; i < n_spectro; ++i) {
-      SavedSpectro s;
-      s.center = r.get<int32_t>();
-      s.counter = r.get<int32_t>();
-      s.last_send = r.get<int64_t>();
-      s.sum = r.span(sizeof(float) * M);
-      if (!r.ok || s.counter < 0 || (i > 0 && s.center <= s_spectro.back().center)) return bad("the spectrogram section is malformed");
-      s_spectro.push_back(s);
-    }
-    if (!r.close()) return bad("the spectrogram section has the wrong length");
-
-    if (!r.open(state_tag("AVGR"))) return bad("the Averager section is missing or truncated");
-    const int32_t s_avg_frames = r.get<int32_t>();
-    const uint8_t* s_sum = r.span(sizeof(float) * n);
-    const uint8_t* s_avg = r.span(sizeof(float) * n);
-    const uint8_t* s_ring = r.span(sizeof(float) * n * Y);
-    if (!r.close() || s_avg_frames < 0 || s_avg_frames > Y) return bad("the Averager section is malformed");
-
-    if (!r.open(state_tag("SMAP"))) return bad("the signal map section is missing or truncated");
-    const int32_t s_live = r.get<int32_t>();
-    if (s_live < 0 || s_live > n || !r.fits(s_live, sizeof(int) + 2 * sizeof(long long) + sizeof(float))) return bad("the signal map section is malformed");
-    const uint8_t* s_keys = r.span(sizeof(int) * s_live);
-    const uint8_t* s_first = r.span(sizeof(long long) * s_live);
-    const uint8_t* s_last = r.span(sizeof(long long) * s_live);
-    const uint8_t* s_power = r.span(sizeof(float) * s_live);
-    if (!r.close()) return bad("the signal map section has the wrong length");
-    {
-      std::vector<int> keys(s_live);
-      if (s_live > 0) std::memcpy(keys.data(), s_keys, sizeof(int) * s_live);
-      for (int i = 0; i < s_live; ++i) {
-        if (keys[i] < 0 || keys[i] >= n || (i > 0 && keys[i] <= keys[i - 1])) return bad("the signal map's keys are not strictly ascending bins");
-      }
-    }
-
-    if (!r.open(state_tag("MBOX"))) return bad("the mailbox section is missing or truncated");
-    const uint32_t s_mail = r.get<uint32_t>();
-    if (s_mail > static_cast<uint32_t>(n) || !r.fits(s_mail, sizeof(b2s_transmission))) return bad("the mailbox section is malformed");
-    std::vector<b2s_transmission> s_mailbox(s_mail);
-    for (b2s_transmission& t : s_mailbox) {
-      t.shift_hz = r.get<int32_t>(), t.flush = r.get<int32_t>(), t.key = r.get<int32_t>(), t.power = r.get<float>();
-    }
-    if (!r.close()) return bad("the mailbox section has the wrong length");
-
-    if (!r.open(state_tag("EVNT"))) return bad("the event section is missing or truncated");
-    const uint64_t s_n_events = r.get<uint64_t>();
-    if (!r.fits(s_n_events, 48)) return bad("the event section is truncated");
-    std::deque<b2s_signal_event> s_events(s_n_events);
-    for (b2s_signal_event& e : s_events) {
-      e.kind = r.get<int32_t>(), e.key = r.get<int32_t>(), e.shift_hz = r.get<int32_t>(), e.reserved = r.get<int32_t>();
-      e.frame = r.get<int64_t>(), e.time_ms = r.get<int64_t>(), e.first_ms = r.get<int64_t>(), e.last_ms = r.get<int64_t>();
-    }
-    if (!r.close()) return bad("the event section has the wrong length");
-
-    if (!r.open(state_tag("ROWS"))) return bad("the spectrogram row section is missing or truncated");
-    const uint64_t s_n_rows = r.get<uint64_t>();
-    if (!r.fits(s_n_rows, 12 + M) || (M == 0 && s_n_rows > 0)) return bad("the spectrogram row section is malformed");
-    std::vector<SentRow> s_sent(s_n_rows);
-    for (SentRow& s : s_sent) {
-      s.time = r.get<int64_t>();
-      s.center = r.get<int32_t>();
-      const uint8_t* row = r.span(M);
-      if (row) s.row.assign(reinterpret_cast<const int8_t*>(row), reinterpret_cast<const int8_t*>(row) + M);
-    }
-    if (!r.close()) return bad("the spectrogram row section has the wrong length");
-    if (r.at != r.end) return bad("unexpected bytes after the last section");
+    snapshot::BandImage s;
+    std::vector<b2s_transmission> s_mailbox;
+    std::deque<b2s_signal_event> s_events;
+    std::vector<SentRow> s_sent;
+    if ((rc = snapshot::read(buf, len, snapshot::kBand, "b2s_band_load_state", [&](snapshot::Reader& r) {
+           snapshot::band_sections(r, s, s_mailbox, s_events, s_sent, cfg, user_window.data());
+         })))
+      return rc;
+    const size_t n = cfg.fft_size, Y = cfg.grouping_y, M = std::max(cfg.spectrogram_out_size, 0);
 
     // ---- allocate: the new noise and spectrogram slots, and the larger entry lists ----
     std::map<int32_t, NoiseSlot> new_noise;
-    for (const SavedNoise& s : s_noise) {
-      NoiseSlot& ns = new_noise[s.center];
+    for (const snapshot::NoiseImage& x : s.noise) {
+      NoiseSlot& ns = new_noise[x.center];
       if ((rc = alloc_noise(ns))) return rc;
-      ns.samples = s.samples;
-      ns.ready = s.ready;
-      ns.started = s.started;
-      ns.start_ms = s.start_ms;
+      ns.samples = x.samples, ns.ready = x.ready, ns.started = x.started, ns.start_ms = x.start_ms;
     }
     std::map<int32_t, SpectroSlot> new_spectro;
-    for (const SavedSpectro& s : s_spectro) {
-      SpectroSlot& ss = new_spectro[s.center];
+    for (const snapshot::SpectroImage& x : s.spectro) {
+      SpectroSlot& ss = new_spectro[x.center];
       if ((rc = ss.sum.alloc(M))) return rc;
-      ss.counter = s.counter;
-      ss.last_send = s.last_send;
+      ss.counter = x.counter, ss.last_send = x.last_send;
     }
     const int wanted_before = wanted_capacity;
-    wanted_capacity = std::max(wanted_capacity, static_cast<int>(s_cap));
+    wanted_capacity = std::max(wanted_capacity, s.capacity);
     if ((rc = grow_capacity())) {
       wanted_capacity = wanted_before;
       return rc;
     }
 
     // ---- replace ----
-    for (const SavedNoise& s : s_noise) CU(cudaMemcpyAsync(new_noise[s.center].threshold[0].p, s.thr, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
-    for (const SavedSpectro& s : s_spectro) CU(cudaMemcpyAsync(new_spectro[s.center].sum.p, s.sum, sizeof(float) * M, cudaMemcpyHostToDevice, stream));
-    CU(cudaMemcpyAsync(d_sum[sum_cur].p, s_sum, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
-    CU(cudaMemcpyAsync(d_avg_last.p, s_avg, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
-    CU(cudaMemcpyAsync(d_ring[ring_cur].p, s_ring, sizeof(float) * n * Y, cudaMemcpyHostToDevice, stream));
-    if (s_live > 0) {
-      CU(cudaMemcpyAsync(d_map_key.p, s_keys, sizeof(int) * s_live, cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_map_first.p, s_first, sizeof(long long) * s_live, cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_map_last.p, s_last, sizeof(long long) * s_live, cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_map_power.p, s_power, sizeof(float) * s_live, cudaMemcpyHostToDevice, stream));
-    }
-    CU(cudaMemcpyAsync(d_map_n.p, &s_live, sizeof(int), cudaMemcpyHostToDevice, stream));
+    for (const snapshot::NoiseImage& x : s.noise) CU(cudaMemcpyAsync(new_noise[x.center].threshold[0].p, x.thr, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
+    for (const snapshot::SpectroImage& x : s.spectro) CU(cudaMemcpyAsync(new_spectro[x.center].sum.p, x.sum, sizeof(float) * M, cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(d_sum[sum_cur].p, s.avg_sum, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(d_avg_last.p, s.avg_last, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(d_ring[ring_cur].p, s.ring, sizeof(float) * n * Y, cudaMemcpyHostToDevice, stream));
+    const size_t live = s.live;
+    CU(cudaMemcpyAsync(d_map_key.p, s.key, sizeof(int) * live, cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(d_map_first.p, s.first, sizeof(long long) * live, cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(d_map_last.p, s.last, sizeof(long long) * live, cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(d_map_power.p, s.power, sizeof(float) * live, cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(d_map_n.p, &s.live, sizeof(int), cudaMemcpyHostToDevice, stream));
     CU(cudaStreamSynchronize(stream));  // K4 reads the map on track_stream, which waits for `stream` in every push
     noise.swap(new_noise);
     spectro.swap(new_spectro);
-    center = s_center;
-    tracker.p.center = s_center;
-    tracker.p.range_lo = s_lo;
-    tracker.p.range_hi = s_hi;
+    center = tracker.p.center = s.center, tracker.p.range_lo = s.range_lo, tracker.p.range_hi = s.range_hi, frames_pushed = s.frames_pushed;
+    event_log = s.event_log, stat_entries = s.stat_entries, stat_rows = s.stat_rows, avg_frames = s.avg_frames;
     tracker.signals.clear();
-    frames_pushed = s_frames;
-    event_log = s_log;
-    stat_entries = s_entries;
-    stat_rows = s_rows;
-    avg_frames = s_avg_frames;
     sent.swap(s_sent);
+    // the frames pushed before belong to another stream: so do the bank history's pieces, auto-record and its START records
+    hist_pieces.clear();
+    autorec = AutoRecord{};
     std::lock_guard<std::mutex> lk(qmutex);
     mailbox.swap(s_mailbox);
     events.swap(s_events);
+    start_of.clear();
     return 0;
   }
 

@@ -46,11 +46,11 @@ def batch_scene(k):
     return Scene(tones, [100, 200], n_ch=k, hist_frames=253, sigma=2.0, max_frames=64, rec_bw=8_000, n_fft=4096)
 
 
-_IQ = {}
+_IQ = {}  # keyed by the Scene itself, which the key keeps alive, so that no later scene can reuse its id()
 
 
 def scene_iq(scene, r, fmt):
-    key = (id(scene), r, fmt)
+    key = (scene, r, fmt)
     if key not in _IQ:
         n_fft = scene.n_fft
         stride = n_fft * r

@@ -434,3 +434,75 @@ def test_snapshot_with_other_user_window_taps_is_refused(engine):
     same.load_state(blob)  # equal taps from another array are accepted
     assert same.save_state() == blob
     same.close()
+
+
+# ---- every section cut short, and every list count forged ----
+def sections(blob):
+    """[(tag, start of the payload, payload length)] of a snapshot, found from the framing alone (u32 tag, u64 length)."""
+    out, at, end = [], 20, len(blob) - 8
+    while at < end:
+        tag, n = struct.unpack_from("<4sQ", blob, at)
+        out.append((tag.decode(), at + 12, n))
+        at += 12 + n
+    assert at == end
+    return out
+
+
+def variants(blob, counts):
+    """(what, snapshot): each section's payload cut by one byte, and each list count that `counts(tag, payload)` locates as
+    (offset, struct format) raised to count + 1 and to 2^32 - 1; the section length, the total length and the checksum fixed up."""
+    for tag, start, n in sections(blob):
+        payload = blob[start : start + n]
+        changed = [(f"{tag} cut by one byte", payload[:-1])]
+        for off, fmt in counts(tag, payload):
+            for v in (struct.unpack_from(fmt, payload, off)[0] + 1, 2**32 - 1):
+                p = bytearray(payload)
+                struct.pack_into(fmt, p, off, v)
+                changed.append((f"{tag} count at {off} set to {v}", bytes(p)))
+        for what, p in changed:
+            body = blob[: start - 8] + struct.pack("<Q", len(p)) + p + blob[start + n : -8]
+            yield what, resealed(body[:12] + struct.pack("<Q", len(body) + 8) + body[20:])
+
+
+def test_every_section_cut_or_with_a_forged_count_is_refused(engine):
+    feed = Feed(scene(400))
+    a = b2s.Band(engine, config())
+    a.set_event_log(True)
+    for f0, nf in ((0, 60), (60, 120)):
+        feed.push(a, f0, nf)
+    blob = a.save_state()
+    a.close()
+    assert [t for t, _, _ in sections(blob)] == ["CONF", "SCAL", "NOIS", "SPEC", "AVGR", "SMAP", "MBOX", "EVNT", "ROWS"]
+    band_counts = {"NOIS": "<I", "SPEC": "<I", "SMAP": "<I", "MBOX": "<I", "EVNT": "<Q", "ROWS": "<Q"}  # each at the payload's start
+    for what, x in variants(blob, lambda tag, payload: [(0, band_counts[tag])] if tag in band_counts else []):
+        try:
+            assert_refused(engine, config(), x, feed, 180)
+        except BaseException as e:
+            raise AssertionError(what) from e
+
+    bank = b2s.RecorderBank(engine, FS, BW, 3)
+    bank.start(0, 317_500)
+    bank.start(1, 0)  # channel 2 stays idle
+    bank.push(feed.iq)
+    kblob = bank.save_state()
+    chunk_bytes = len(bank.flush(0, cap=1, consume=False)[0][1])
+    chan = [(start, n) for t, start, n in sections(kblob) if t == "CHAN"]
+    assert [t for t, _, _ in sections(kblob)] == ["CONF", "RAWC"] + ["CHAN"] * 3
+    carry = chan[2][1] - 50  # the idle channel: 2 bool bytes, 4 x 8 bytes, its carries, a chunk count of 0 and a tail of 0 (u64 each)
+
+    def chan_counts(tag, payload):
+        if tag != "CHAN":
+            return []
+        at = 34 + carry
+        n = struct.unpack_from("<Q", payload, at)[0]
+        return [(at, "<Q"), (at + 8 + n * chunk_bytes, "<Q")]  # the complete chunks, the tail's bytes
+
+    assert struct.unpack_from("<Q", kblob, chan[0][0] + 34 + carry)[0] > 0, "channel 0 holds no complete chunk"
+    for what, x in variants(kblob, chan_counts):
+        try:
+            with pytest.raises(b2s.B2SError, match=INVALID):
+                bank.load_state(x)
+            assert bank.save_state() == kblob
+        except BaseException as e:
+            raise AssertionError(what) from e
+    bank.close()
