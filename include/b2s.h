@@ -240,6 +240,34 @@ int b2s_band_set_event_log(b2s_band* b, int enable);
  * events copied out (and only those) are dropped from the log */
 int b2s_band_get_events(b2s_band* b, b2s_signal_event* out, int cap, int consume, int* count);
 
+/* ---- spectrum occupancy: how often each bin is busy, and how strong it gets, per centre frequency ----
+ * Accumulated on the device over the pushes since occupancy was enabled or the centre's statistics were last reset, so a band that runs
+ * all day can tell which frequencies are busy and for how much of the time (to choose start_level, stop_level, the scanned ranges and
+ * ignored ranges) without dense debug rows.
+ *   - Per centre: a centre's statistics (3 x N x 4 B of device memory) are allocated the first time a push runs at that centre with
+ *     occupancy on. They count only the frames pushed at that centre.
+ *   - frames: every frame pushed at the centre while occupancy was on. detect_frames: those past noise learning, the frames the
+ *     detector produces entries for.
+ *   - above_start[b] / above_stop[b]: the detect frames whose boxcar value (b2s_result.box_db) of bin b is >= start_level / >= stop_level,
+ *     decided on the detection entries with the predicate the signal bookkeeping uses. Every bin counts: the scanned range and the
+ *     ignored ranges do not apply. above_start[b] / detect_frames is bin b's duty cycle at the start level.
+ *   - max_db[b]: the largest raw PSD value (b2s_result.psd_db, after sub-frame folding) of bin b over all `frames`, learning frames
+ *     included; -inf before the first frame.
+ *   - truncated: the pieces of pushes (b2s_band_push works in pieces of at most max_frames_per_push frames) whose detection lists
+ *     overflowed detect_capacity (the push returned B2S_E_OVERFLOW) among those counted. While it is nonzero, above_start and above_stop
+ *     are lower bounds.
+ *   - The counters are 32-bit and wrap after 2^32 frames (2.7 years at 50 frames/s).
+ * The band's own results (mailbox, map, spectrogram rows, events, Averager, noise, an attached bank's output) are bit for bit those of
+ * the same band with occupancy off. b2s_band_reset and b2s_band_set_center clear nothing. Occupancy is not part of a snapshot. */
+/* enable != 0: the pushes after this call are counted (off by default); turning it off keeps what was accumulated, readable as before */
+int b2s_band_set_occupancy(b2s_band* b, int enable);
+/* the centres with statistics, ascending: up to `cap` are copied, *count is the number there are */
+int b2s_band_occupancy_centers(b2s_band* b, int32_t* centers_hz, int cap, int* count);
+/* The statistics of one centre. Outstanding pushes are finished first (as b2s_band_save_state does). With reset != 0 the centre's counts
+ * and max-hold are cleared after they are copied out. Every pointer is required; B2S_E_INVALID for a centre without statistics. */
+int b2s_band_get_occupancy(b2s_band* b, int32_t center_hz, uint32_t* above_start /*[N]*/, uint32_t* above_stop /*[N]*/, float* max_db /*[N]*/,
+                           int64_t* frames, int64_t* detect_frames, int64_t* truncated, int reset);
+
 /* ---- snapshots: save a band's whole state and restore it into another band, in this process or another, on any engine ----
  * A band restored from a snapshot continues exactly like the band that saved it: the noise thresholds of every centre visited, the
  * Averager, the live signals, the spectrogram accumulators, the frame counter of the event log, the current centre and range, the

@@ -10,7 +10,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import weakref
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import numpy as np
 
@@ -236,8 +236,13 @@ def lib():
         L.b2s_band_record_from.argtypes = [C.c_void_p, C.c_int, C.c_int32, C.c_int64]
         L.b2s_band_set_auto_record.argtypes = [C.c_void_p, C.c_int, C.c_int32]
         L.b2s_band_get_auto_record_actions.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int)]
+        L.b2s_band_set_occupancy.argtypes = [C.c_void_p, C.c_int]
+        L.b2s_band_occupancy_centers.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
+        L.b2s_band_get_occupancy.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                             C.POINTER(C.c_int64), C.c_int]
         for f in ("b2s_recorder_bank_set_history", "b2s_recorder_bank_history", "b2s_recorder_bank_start_from", "b2s_band_record_from",
-                  "b2s_band_set_auto_record", "b2s_band_get_auto_record_actions"):
+                  "b2s_band_set_auto_record", "b2s_band_get_auto_record_actions", "b2s_band_set_occupancy", "b2s_band_occupancy_centers",
+                  "b2s_band_get_occupancy"):
             getattr(L, f).restype = C.c_int
         for f in ("b2s_band", "b2s_recorder_bank"):
             getattr(L, f + "_save_state").argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -400,6 +405,17 @@ class Averager(_Handle):
         frames = C.c_int32()
         _check(lib().b2s_averager_sum(self._h, _ptr(out), C.byref(frames)))
         return out, frames.value
+
+
+class Occupancy(NamedTuple):
+    """One centre's spectrum occupancy (b2s_band_get_occupancy). above_start / detect_frames is each bin's duty cycle at the start
+    level; while `truncated` is nonzero the counts are lower bounds."""
+    above_start: np.ndarray  # uint32 [N]
+    above_stop: np.ndarray   # uint32 [N]
+    max_db: np.ndarray       # float32 [N]
+    frames: int
+    detect_frames: int
+    truncated: int
 
 
 class PushOutput:
@@ -579,6 +595,26 @@ class Band(_Handle):
         count = C.c_int()
         _check(lib().b2s_band_get_auto_record_actions(self._h, C.cast(acts, C.c_void_p), cap, 1 if consume else 0, C.byref(count)))
         return [acts[i].astuple() for i in range(min(count.value, cap))]
+
+    def set_occupancy(self, enable: bool = True):
+        """b2s_band_set_occupancy: count the spectrum occupancy of the pushes after this call, per centre frequency."""
+        _check(lib().b2s_band_set_occupancy(self._h, 1 if enable else 0))
+
+    def occupancy_centers(self, cap: int = 1024):
+        """The centres (Hz) with occupancy statistics, ascending."""
+        out = np.zeros(max(cap, 1), dtype=np.int32)
+        count = C.c_int()
+        _check(lib().b2s_band_occupancy_centers(self._h, _ptr(out), cap, C.byref(count)))
+        return [int(c) for c in out[: min(count.value, cap)]]
+
+    def occupancy(self, center_hz: int, reset: bool = False) -> Occupancy:
+        """b2s_band_get_occupancy: one centre's per-bin counts above the start and stop levels, its max-hold trace and frame counts."""
+        n = self.cfg.fft_size
+        o = Occupancy(np.zeros(n, np.uint32), np.zeros(n, np.uint32), np.zeros(n, np.float32), 0, 0, 0)
+        frames, detect, truncated = C.c_int64(), C.c_int64(), C.c_int64()
+        _check(lib().b2s_band_get_occupancy(self._h, center_hz, _ptr(o.above_start), _ptr(o.above_stop), _ptr(o.max_db), C.byref(frames), C.byref(detect),
+                                            C.byref(truncated), 1 if reset else 0))
+        return o._replace(frames=frames.value, detect_frames=detect.value, truncated=truncated.value)
 
     def save_state(self) -> bytes:
         """b2s_band_save_state: the band's whole state as an opaque snapshot (outstanding pushes are finished first)."""

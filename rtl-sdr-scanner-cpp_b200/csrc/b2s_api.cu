@@ -24,6 +24,7 @@
 #include "../../include/b2s.h"
 #include "detect.cuh"
 #include "host_utils.h"
+#include "occupancy.cuh"
 #include "recorder.cuh"
 #include "scan_policy.h"
 #include "spectral3.cuh"
@@ -1602,6 +1603,51 @@ int b2s_band_get_events(b2s_band* b, b2s_signal_event* out, int cap, int consume
   if (rc) return rc;
   std::lock_guard<std::mutex> lk(b->qmutex);
   hand_out_events(b->events, out, cap, consume, count);
+  return 0;
+}
+
+int b2s_band_set_occupancy(b2s_band* b, int enable) {
+  if (!b) return fail(B2S_E_INVALID, "b2s_band_set_occupancy: NULL band");
+  std::lock_guard<std::mutex> lock(b->mutex);
+  b->occupancy = enable != 0;  // read at enqueue time: the pushes after this call
+  return 0;
+}
+
+int b2s_band_occupancy_centers(b2s_band* b, int32_t* centers_hz, int cap, int* count) {
+  if (!b || !count || (!centers_hz && cap > 0)) return fail(B2S_E_INVALID, "b2s_band_occupancy_centers: NULL argument");
+  std::lock_guard<std::mutex> lock(b->mutex);
+  int i = 0;
+  for (const auto& kv : b->occ) {
+    if (i < cap) centers_hz[i] = kv.first;
+    ++i;
+  }
+  *count = i;
+  return 0;
+}
+
+int b2s_band_get_occupancy(b2s_band* b, int32_t center_hz, uint32_t* above_start, uint32_t* above_stop, float* max_db, int64_t* frames,
+                           int64_t* detect_frames, int64_t* truncated, int reset) {
+  const char* who = "b2s_band_get_occupancy";
+  if (!b || !above_start || !above_stop || !max_db || !frames || !detect_frames || !truncated) return fail(B2S_E_INVALID, "%s: NULL argument", who);
+  std::lock_guard<std::mutex> lock(b->mutex);
+  auto it = b->occ.find(center_hz);
+  if (it == b->occ.end()) return fail(B2S_E_INVALID, "%s: no occupancy was counted at centre %d Hz", who, center_hz);
+  CU(cudaSetDevice(b->engine->device));
+  int rc = b->drain();
+  if (rc) return rc;
+  CU(cudaStreamSynchronize(b->stream));
+  OccupancySlot& o = it->second;
+  const size_t n = b->cfg.fft_size;
+  CU(cudaMemcpy(above_start, o.above_start.p, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(above_stop, o.above_stop.p, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(max_db, o.max_db.p, sizeof(float) * n, cudaMemcpyDeviceToHost));
+  *frames = o.frames;
+  *detect_frames = o.detect_frames;
+  *truncated = o.truncated;
+  if (reset) {
+    if ((rc = b->clear_occupancy(o))) return rc;
+    CU(cudaStreamSynchronize(b->stream));  // cleared before the call returns, whichever stream the next push uses
+  }
   return 0;
 }
 

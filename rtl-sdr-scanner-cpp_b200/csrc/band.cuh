@@ -31,6 +31,13 @@ struct SpectroSlot {
   int counter = 0;
   int64_t last_send = 0;
 };
+// spectrum occupancy of one centre (b2s_band_set_occupancy): the device counts and max-hold, and the host's frame counts
+struct OccupancySlot {
+  DevBuf<unsigned int> above_start, above_stop;  // [N]
+  DevBuf<float> max_db;                          // [N]
+  int64_t frames = 0, detect_frames = 0;
+  int64_t truncated = 0;  // counted chunks whose entry lists overflowed detect_capacity (written by the finish half, under qmutex)
+};
 struct SentRow {
   int64_t time;
   int32_t center;
@@ -60,6 +67,7 @@ struct PushSlot {
   bool log_on = false;       // the event log was on when the chunk was enqueued
   bool log_starts = false;   // auto-record was on: K4 logs even with the event log off, and the STARTs go to the band's start_of
   int64_t frame_base = 0;    // frames pushed to the band before the chunk's first
+  OccupancySlot* occ = nullptr;  // the centre's occupancy slot when occupancy was on at enqueue time
   Event sorted_done, tev[2];
   bool host_track = false;  // this chunk's bookkeeping runs on the host (the caller asked for every frame's list)
   int epoch = 0;            // reset_epoch when the chunk was enqueued
@@ -166,6 +174,9 @@ struct b2s_band : public DeviceQueries {
 
   std::map<int32_t, NoiseSlot> noise;
   std::map<int32_t, SpectroSlot> spectro;
+  // spectrum occupancy (off by default): one slot per centre pushed while it was on; turning it off keeps them. Not in a snapshot.
+  bool occupancy = false;
+  std::map<int32_t, OccupancySlot> occ;
   std::vector<SentRow> sent;
   int32_t center = 0;
   Tracker tracker;
@@ -215,6 +226,32 @@ struct b2s_band : public DeviceQueries {
       std::vector<float> init(cfg.fft_size, -std::numeric_limits<float>::max());  // noise_learner.cpp:16
       CU(cudaMemcpyAsync(it->second.threshold[0].p, init.data(), sizeof(float) * cfg.fft_size, cudaMemcpyHostToDevice, stream));
       CU(cudaStreamSynchronize(stream));
+    }
+    *out = &it->second;
+    return 0;
+  }
+  // counts zeroed, max-hold -inf, on `stream` (the next push's occupancy kernels follow in stream order)
+  int clear_occupancy(OccupancySlot& o) {
+    const size_t n = cfg.fft_size;
+    CU(cudaMemsetAsync(o.above_start.p, 0, sizeof(unsigned int) * n, stream));
+    CU(cudaMemsetAsync(o.above_stop.p, 0, sizeof(unsigned int) * n, stream));
+    k_fill<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(o.max_db.p, -INFINITY, static_cast<int>(n));
+    CU(cudaGetLastError());
+    o.frames = o.detect_frames = o.truncated = 0;
+    return 0;
+  }
+  // the current centre's occupancy slot, allocated and cleared on the first push at that centre
+  int occupancy_slot(OccupancySlot** out) {
+    auto it = occ.find(center);
+    if (it == occ.end()) {
+      OccupancySlot o;
+      const size_t n = cfg.fft_size;
+      int rc = o.above_start.alloc(n);
+      if (!rc) rc = o.above_stop.alloc(n);
+      if (!rc) rc = o.max_db.alloc(n);
+      if (!rc) rc = clear_occupancy(o);
+      if (rc) return rc;
+      it = occ.emplace(center, std::move(o)).first;
     }
     *out = &it->second;
     return 0;
@@ -794,6 +831,8 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
   s.log_on = event_log;
   s.log_starts = autorec.on;
   s.frame_base = frames_pushed;
+  s.occ = nullptr;
+  if (occupancy && (rc = occupancy_slot(&s.occ))) return rc;
   if ((s.log_on || s.log_starts) && !s.host_track && (rc = s.d_log.alloc(n))) return rc;
   if (s.host_track && (rc = state_to_host_tracker())) return rc;
   s.dense_q_on = out && out->noise_sub_db;
@@ -1053,6 +1092,28 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
     CU(cudaEventRecord(s.gpu_done, stream));
   }
 
+  // ---- occupancy: behind the list ordering on `stream`, after the events K4 and the finish half wait for, so neither waits for it.
+  // The slot's PSD rows are next written by the K1 of the push after next, which `stream` runs after these kernels. ----
+  if (s.occ) {
+    OccupancySlot& o = *s.occ;
+    const int learning = std::min(T, std::max(0, da.learn_frames - da.noise_samples));  // frames t with noise_samples + t < learn_frames
+    o.frames += T;
+    o.detect_frames += T - learning;
+    if (T > learning) {
+      const long long bound = static_cast<long long>(T) * slot_capacity;
+      const int grid = static_cast<int>(std::max(1LL, std::min<long long>((bound + 255) / 256, 8LL * engine->sm_count)));
+      k_occupancy_count<<<grid, 256, 0, stream>>>(s.sorted.p, s.offsets.p, T, cfg.start_level, cfg.stop_level, o.above_start.p, o.above_stop.p);
+      CU(cudaGetLastError());
+    }
+    // more row groups per CTA while N / 32 CTAs would leave threads idle (up to 128 x 8 threads, 16 KB of shared memory)
+    const int ctas = n / kOccupancyBins;
+    int groups = 32;
+    while (groups < 128 && static_cast<long long>(ctas) * groups * kOccupancyCols * 2 <= 2048LL * engine->sm_count) groups *= 2;
+    const int threads = groups * kOccupancyCols;
+    k_occupancy_max<<<ctas, threads, sizeof(float4) * threads, stream>>>(s.psd.p, n, T, o.max_db.p);
+    CU(cudaGetLastError());
+  }
+
   // context for the finish half
   s.T = T;
   s.t0_ms = t0_ms;
@@ -1237,6 +1298,10 @@ int b2s_band::finish_chunk(PushSlot& s) {
   }
   CU(cudaStreamSynchronize(st));
   cur = nullptr;
+  if (overflow && s.occ) {  // the occupancy counts of this chunk came from the truncated lists
+    std::lock_guard<std::mutex> lk(qmutex);
+    s.occ->truncated += 1;
+  }
   if (overflow)
     return fail(B2S_E_OVERFLOW, "a frame produced %d detection entries but detect_capacity is %d per frame: the frame's list was truncated (the push completed on the "
                 "truncated lists); the capacity grows to %d before the next push", worst_count, slot_capacity, std::min(cfg.fft_size, wanted_capacity));
