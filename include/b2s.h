@@ -77,6 +77,27 @@ extern "C" {
  * MAX suits bursts shorter than a stride: the mean would dilute a burst that fills one sub-frame by 10 log10(r) dB. */
 #define B2S_FLAG_SUBFRAME_MEAN 0x400
 #define B2S_FLAG_SUBFRAME_MAX 0x800
+/* Overlapping sub-frames (opt-in, with exactly one of B2S_FLAG_SUBFRAME_MEAN / _MAX): back-to-back Hamming sub-frames lose a
+ * burst that sits on a sub-frame edge, where both windows taper to 0.08 (about 28 dB for a tone burst of fft_size / 16 samples).
+ * With h = fft_size / 2 the sub-frames overlap by half, so every sample lies in the central half of exactly one of them.
+ *   - frame_stride_samples must be at least fft_size and a multiple of h (b2s_default_config's strides are); any other use, or the
+ *     flag without exactly one of MEAN / MAX, is refused (B2S_E_INVALID) by b2s_band_create and b2s_psd.
+ *   - Frame k has m = frame_stride_samples / h sub-frames; sub-frame j (j = 0 ... m-1) is the fft_size samples starting at
+ *     k * frame_stride_samples - h + j * h. Sub-frame 0 straddles the end of the previous frame, sub-frame m-1 ends with frame k's
+ *     stride, and frame k owns the samples [k * stride - fft_size / 4, (k + 1) * stride - fft_size / 4) (the central halves).
+ *     Each is windowed, transformed, shifted and squared as above and folded in ascending j by MEAN (then divided by the count
+ *     folded) or MAX.
+ *   - The lead-in: frame 0 of a push takes its sub-frame 0's first h samples from the last h samples of the band's previous push,
+ *     which the band keeps on the device. There is none on the first push after b2s_band_create, after a b2s_band_set_center that
+ *     changes the centre, and after a b2s_band_load_state whose snapshot holds none; that frame then folds sub-frames 1 ... m-1
+ *     (MEAN divides by m - 1). b2s_band_reset keeps it: the IQ stream does not break.
+ *   - Input: a push reads n_frames * frame_stride_samples samples, the whole stream (host or device, with or without a bank).
+ *     b2s_psd reads h + n_frames * frame_stride_samples samples: `iq` points at frame 0's lead-in, and every frame folds all m.
+ *   - However a stream is cut into pushes, and however the band cuts a push into pieces, the results are bit for bit the same
+ *     (given the same frame clocks).
+ *   - A band snapshot holds the lead-in (one extra section, only for bands with the flag); a load into a band whose overlap bit
+ *     differs is refused. */
+#define B2S_FLAG_SUBFRAME_OVERLAP 0x1000
 
 /* Construction-time parameters. The reference takes them from Config / Device / the setupChains lambdas
  * (sdr_device.cpp:148-167, transmission.h:17-25, config.h:24-38). */

@@ -24,6 +24,7 @@ FLAG_IQ_ON_DEVICE = 0x100
 FLAG_ASYNC = 0x200
 FLAG_SUBFRAME_MEAN = 0x400  # a frame's PSD row is the mean of its stride's floor(stride / N) sub-frame periodograms (include/b2s.h)
 FLAG_SUBFRAME_MAX = 0x800   # ... or their per-bin maximum; make_config(flags=...) and Engine.psd pass them through
+FLAG_SUBFRAME_OVERLAP = 0x1000  # with MEAN or MAX: stride / (N / 2) sub-frames overlapping by half; Engine.psd then reads a lead-in
 
 
 class BandConfig(C.Structure):
@@ -366,6 +367,11 @@ class Engine(_Handle):
         psd = np.empty((n_frames, n), dtype=np.float32)
         lin = np.empty((n_frames, n), dtype=np.float32) if want_linear else None
         iq = np.ascontiguousarray(iq)
+        if cfg.flags & FLAG_SUBFRAME_OVERLAP:
+            # N / 2 lead-in samples, then every frame's whole stride (include/b2s.h)
+            need = (n // 2 + n_frames * cfg.frame_stride_samples) * (2 if cfg.iq_format == IQ_CS8 else 8)
+            if iq.nbytes < need:
+                raise ValueError(f"overlapping sub-frames read {need} bytes of IQ; {iq.nbytes} were given")
         _check(lib().b2s_psd(self._h, C.byref(cfg), _ptr(iq), n_frames, _ptr(psd), _ptr(lin)))
         return (psd, lin) if want_linear else psd
 

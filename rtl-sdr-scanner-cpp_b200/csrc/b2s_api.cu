@@ -295,9 +295,21 @@ void plan_radices(int n, int* r) {
   }
 }
 
-// Sub-frames a frame's PSD row is made of: floor(stride / N) with B2S_FLAG_SUBFRAME_MEAN or _MAX, else 1.
+// Sub-frames a frame's PSD row is made of: floor(stride / N) with B2S_FLAG_SUBFRAME_MEAN or _MAX, stride / (N / 2) when they overlap
+// by half (B2S_FLAG_SUBFRAME_OVERLAP), else 1.
 constexpr int kSubframeFlags = B2S_FLAG_SUBFRAME_MEAN | B2S_FLAG_SUBFRAME_MAX;
-int subframes(const b2s_band_config& c) { return (c.flags & kSubframeFlags) ? c.frame_stride_samples / c.fft_size : 1; }
+bool overlapped(const b2s_band_config& c) { return (c.flags & B2S_FLAG_SUBFRAME_OVERLAP) != 0; }
+int subframes(const b2s_band_config& c) {
+  if (!(c.flags & kSubframeFlags)) return 1;
+  return overlapped(c) ? c.frame_stride_samples / (c.fft_size / 2) : c.frame_stride_samples / c.fft_size;
+}
+// Samples a push of n >= 1 frames reads: its last frame needs its sub-frames only, unless they overlap (the last one ends with the
+// stride) or `whole` (an attached bank reads the whole stream)
+size_t push_samples(const b2s_band_config& c, size_t n, bool whole) {
+  const size_t stride = static_cast<size_t>(c.frame_stride_samples);
+  if (whole || overlapped(c)) return n * stride;
+  return (n - 1) * stride + static_cast<size_t>(subframes(c)) * c.fft_size;
+}
 
 struct SpectralTables {
   DevBuf<float> wscale;
@@ -305,10 +317,14 @@ struct SpectralTables {
   DevBuf<int> work_counter;  // k_spectrum3's {next item, finished CTAs}; the kernel leaves both at zero
   int split = 1;
   int sub_r = 1, sub_max = 0;  // sub-frames per frame and their reduction (B2S_FLAG_SUBFRAME_*)
+  long long sub_step = 0, sub_off = 0;  // where they lie (SpectralArgs::sub_step_bytes, sub_off_bytes)
   int build(const b2s_band_config& cfg) {
     const int n = cfg.fft_size;
     sub_r = subframes(cfg);
     sub_max = (cfg.flags & B2S_FLAG_SUBFRAME_MAX) != 0;
+    const long long bps = cfg.iq_format == B2S_IQ_CS8 ? 2 : 8;
+    sub_step = (overlapped(cfg) ? n / 2 : n) * bps;
+    sub_off = overlapped(cfg) ? -(n / 2) * bps : 0;
     std::vector<float> w;
     make_window(cfg, w);
     if (cfg.iq_format == B2S_IQ_CS8) {
@@ -372,6 +388,8 @@ struct SpectralTables {
     sa.split_ws = split_ws.p;
     sa.sub_r = sub_r;
     sa.sub_max = sub_max;
+    sa.sub_step_bytes = sub_step;
+    sa.sub_off_bytes = sub_off;
   }
 };
 
@@ -384,6 +402,10 @@ int validate_config(const b2s_band_config& c) {
   if (c.frame_stride_samples < c.fft_size) return fail(B2S_E_INVALID, "frame_stride_samples (%d) < fft_size", c.frame_stride_samples);
   if (c.iq_format != B2S_IQ_CS8 && c.iq_format != B2S_IQ_CF32) return fail(B2S_E_INVALID, "unknown iq_format %d", c.iq_format);
   if ((c.flags & kSubframeFlags) == kSubframeFlags) return fail(B2S_E_INVALID, "B2S_FLAG_SUBFRAME_MEAN and B2S_FLAG_SUBFRAME_MAX exclude each other");
+  if (overlapped(c) && !(c.flags & kSubframeFlags))
+    return fail(B2S_E_INVALID, "B2S_FLAG_SUBFRAME_OVERLAP needs B2S_FLAG_SUBFRAME_MEAN or B2S_FLAG_SUBFRAME_MAX");
+  if (overlapped(c) && c.frame_stride_samples % (c.fft_size / 2) != 0)
+    return fail(B2S_E_INVALID, "B2S_FLAG_SUBFRAME_OVERLAP needs a frame_stride_samples (%d) that is a multiple of fft_size / 2", c.frame_stride_samples);
   if (c.window_kind == B2S_WINDOW_USER && !c.window_taps) return fail(B2S_E_INVALID, "window_taps is NULL");
   if (c.grouping_x < 1 || c.grouping_x > 65) return fail(B2S_E_INVALID, "grouping_x must be in 1..65");
   if (c.grouping_y < 1 || c.grouping_y > 256) return fail(B2S_E_INVALID, "grouping_y must be in 1..256");
@@ -1301,8 +1323,7 @@ static int band_push(b2s_band* b, const void* iq, size_t n_frames, int64_t t0_ms
   auto chunk_len = [&](size_t done) { return std::min(n_frames - done, pipe); };
   auto start_copy = [&](size_t done, int slot) -> int {
     const size_t chunk = chunk_len(done);
-    // the last frame needs its r sub-frames of N samples only (r = 1 without sub-frames), unless a bank reads the whole stream
-    const size_t bytes = b->bank ? chunk * stride_bytes : (chunk - 1) * stride_bytes + static_cast<size_t>(subframes(b->cfg)) * b->cfg.fft_size * bytes_per_sample;
+    const size_t bytes = push_samples(b->cfg, chunk, b->bank != nullptr) * bytes_per_sample;
     CU(cudaMemcpyAsync(b->d_iq[slot].p, static_cast<const char*>(iq) + done * stride_bytes, bytes, cudaMemcpyHostToDevice, b->copy_stream));
     CU(cudaEventRecord(b->copy_done[slot], b->copy_stream));
     b->prof.h2d_bytes += bytes;
@@ -1421,7 +1442,10 @@ int b2s_band_set_center(b2s_band* b, int32_t center_hz, int32_t lo, int32_t hi) 
   std::lock_guard<std::mutex> lock(b->mutex);
   int rc = b->drain();
   if (rc) return rc;
-  if (center_hz != b->center) b->hist_pieces.clear();  // the history's IQ belongs to the old centre
+  if (center_hz != b->center) {
+    b->hist_pieces.clear();  // the history's IQ belongs to the old centre
+    b->has_lead = false;     // and so do the samples before the next push
+  }
   b->center = center_hz;
   b->tracker.p.center = center_hz;
   b->tracker.p.range_lo = lo;
@@ -1746,7 +1770,10 @@ int b2s_psd(b2s_engine* e, const b2s_band_config* cfg, const void* iq, size_t n_
   const size_t n = c.fft_size;
   const size_t bps = c.iq_format == B2S_IQ_CS8 ? 2 : 8;
   const size_t stride = static_cast<size_t>(c.frame_stride_samples) * bps;
-  const size_t bytes = (n_frames - 1) * stride + static_cast<size_t>(subframes(c)) * n * bps;
+  // overlapping sub-frames: `iq` starts with frame 0's lead-in of N / 2 samples, which K1 reads as frame 0's sub-frame 0 along with
+  // the first N / 2 samples of the frame
+  const size_t lead = overlapped(c) ? n / 2 * bps : 0;
+  const size_t bytes = lead + push_samples(c, n_frames, false) * bps;
   rc = tables.build(c);
   if (!rc) rc = diq.alloc(bytes);
   if (!rc) rc = dpsd.alloc(n_frames * n);
@@ -1757,10 +1784,11 @@ int b2s_psd(b2s_engine* e, const b2s_band_config* cfg, const void* iq, size_t n_
   if (rc) return rc;
   CU(cudaMemcpy(diq.p, iq, bytes, cudaMemcpyHostToDevice));
   SpectralArgs sa{};
-  sa.iq = diq.p;
+  sa.iq = diq.p + lead;
   sa.frame_stride_bytes = static_cast<long long>(stride);
   sa.n_frames = static_cast<int>(n_frames);
   tables.fill(sa);
+  if (lead) sa.sub_lead = diq.p;
   sa.inv_fs = 1.0f / static_cast<float>(c.sample_rate_hz);
   sa.psd_db = dpsd.p;
   sa.power_lin = power_lin ? dlin.p : nullptr;

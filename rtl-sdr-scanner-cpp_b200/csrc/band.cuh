@@ -160,6 +160,10 @@ struct b2s_band : public DeviceQueries {
 
   SpectralTables tables;
   DevBuf<unsigned char> d_iq[2];
+  // B2S_FLAG_SUBFRAME_OVERLAP: frame 0's sub-frame 0 of the chunk K1 reads next, N samples: the lead-in (the last N / 2 samples of the
+  // chunk before, kept here in stream order), then the chunk's first N / 2. has_lead: the next chunk's frame 0 has a lead-in.
+  DevBuf<unsigned char> d_lead;
+  bool has_lead = false;
   DevBuf<float> d_sum[2], d_ring[kRings], d_avg_last;  // m_sum: [sum_cur] after the last enqueued push (K2 reads it, writes the other)
   int sum_cur = 0;
   int ring_cur = 0;  // d_ring[ring_cur] = ring after the last enqueued push
@@ -389,6 +393,11 @@ struct b2s_band : public DeviceQueries {
     stream = own_stream;
     int rc = tables.build(c);
     if (rc) return rc;
+    if (overlapped(c)) {
+      const size_t lead_bytes = static_cast<size_t>(c.fft_size) * (c.iq_format == B2S_IQ_CS8 ? 2 : 8);
+      if ((rc = d_lead.alloc(lead_bytes))) return rc;
+      CU(cudaMemset(d_lead.p, 0, lead_bytes));  // a snapshot taken before the first push saves defined bytes
+    }
     if (c.window_kind == B2S_WINDOW_USER) user_window.assign(c.window_taps, c.window_taps + c.fft_size);
     cfg.window_taps = nullptr;
     const size_t n = c.fft_size, Y = c.grouping_y;
@@ -645,6 +654,7 @@ struct b2s_band : public DeviceQueries {
     s.avg_frames = avg_frames, s.avg_sum = d_sum[sum_cur].p, s.avg_last = d_avg_last.p, s.ring = d_ring[ring_cur].p;
     CU(cudaMemcpy(&s.live, d_map_n.p, sizeof(int), cudaMemcpyDeviceToHost));
     s.key = d_map_key.p, s.first = d_map_first.p, s.last = d_map_last.p, s.power = d_map_power.p;
+    s.has_lead = has_lead, s.lead = d_lead.p;
     std::lock_guard<std::mutex> lk(qmutex);
     return snapshot::write(snapshot::kBand, stream, out,
                            [&](snapshot::Writer& w) { snapshot::band_sections(w, s, mailbox, events, sent, cfg, user_window.data()); });
@@ -698,7 +708,9 @@ struct b2s_band : public DeviceQueries {
     CU(cudaMemcpyAsync(d_map_last.p, s.last, sizeof(long long) * live, cudaMemcpyHostToDevice, stream));
     CU(cudaMemcpyAsync(d_map_power.p, s.power, sizeof(float) * live, cudaMemcpyHostToDevice, stream));
     CU(cudaMemcpyAsync(d_map_n.p, &s.live, sizeof(int), cudaMemcpyHostToDevice, stream));
+    if (d_lead.p) CU(cudaMemcpyAsync(d_lead.p, s.lead, d_lead.n / 2, cudaMemcpyHostToDevice, stream));
     CU(cudaStreamSynchronize(stream));  // K4 reads the map on track_stream, which waits for `stream` in every push
+    has_lead = s.has_lead;
     noise.swap(new_noise);
     spectro.swap(new_spectro);
     center = tracker.p.center = s.center, tracker.p.range_lo = s.range_lo, tracker.p.range_hi = s.range_hi, frames_pushed = s.frames_pushed;
@@ -863,9 +875,19 @@ int b2s_band::enqueue_chunk(PushSlot& s, const void* iq_dev, size_t frames, int6
   sa.zero_per_frame[0] = d_slot_count.p;  // K2's per-frame counters are zeroed by K1 (no memsets between the two kernels)
   sa.zero_per_frame[1] = s.cand_flag.p;
   sa.zero_scalar = s.max_count.p;
+  const size_t half_bytes = static_cast<size_t>(n / 2) * bytes_per_sample;
+  if (d_lead.p) {  // overlapping sub-frames: frame 0's sub-frame 0 is the lead-in and the chunk's first N / 2 samples, or is dropped
+    CU(cudaMemcpyAsync(d_lead.p + half_bytes, iq_dev, half_bytes, cudaMemcpyDeviceToDevice, stream));
+    sa.sub_lead = has_lead ? d_lead.p : nullptr;
+    sa.sub_first = has_lead ? 0 : 1;
+  }
   if (profiling) CU(cudaEventRecord(s.ev[0], stream));
   if ((rc = launch_spectrum(engine, n, cfg.iq_format, sa, stream))) return rc;
   if (profiling) CU(cudaEventRecord(s.ev[1], stream));
+  if (d_lead.p) {  // the next chunk's lead-in: this one's last N / 2 samples, behind this K1's reads of d_lead
+    CU(cudaMemcpyAsync(d_lead.p, static_cast<const char*>(iq_dev) + T * sa.frame_stride_bytes - half_bytes, half_bytes, cudaMemcpyDeviceToDevice, stream));
+    has_lead = true;
+  }
 
   // ---- plan the spectrogram emissions of this chunk from the clock (Spectrogram::send, spectrogram.cpp:62-75) ----
   int n_emit = 0;

@@ -187,7 +187,7 @@ int read(const void* buf, size_t len, uint32_t kind, const char* who, F&& descri
   return 0;
 }
 
-// ---- band: CONF SCAL NOIS SPEC AVGR SMAP MBOX EVNT ROWS ----
+// ---- band: CONF SCAL NOIS SPEC AVGR SMAP MBOX EVNT ROWS, and LEAD with B2S_FLAG_SUBFRAME_OVERLAP ----
 // every field of b2s_band_config except the window_taps pointer, in declaration order
 template <typename F>
 void band_config_fields(b2s_band_config& c, F&& f) {
@@ -199,12 +199,13 @@ void band_config_fields(b2s_band_config& c, F&& f) {
   f(c.max_frames_per_push), f(c.detect_capacity), f(c.noise_learning_ms);
 }
 // Two creation configs that a snapshot may move between: equal bit for bit except the centre and range (state), the flags other
-// than the sub-frame bits (the learned noise depends on those) and the sizing fields.
+// than the sub-frame bits (the learned noise depends on those, and the overlap bit on whether the snapshot holds a lead-in) and the
+// sizing fields.
 inline bool same_band_config(b2s_band_config a, b2s_band_config b) {
   Writer x, y;
   for (auto* c : {&a, &b}) {
     c->center_hz = c->range_lo_hz = c->range_hi_hz = c->max_frames_per_push = c->detect_capacity = 0;
-    c->flags &= kSubframeFlags;
+    c->flags &= kSubframeFlags | B2S_FLAG_SUBFRAME_OVERLAP;
     c->window_taps = nullptr;
   }
   band_config_fields(a, x);
@@ -236,6 +237,8 @@ struct BandImage {
   const void *avg_sum = nullptr, *avg_last = nullptr, *ring = nullptr;  // [N], [N], [Y][N] oldest row first
   int32_t live = 0;  // the signal map: its live entries, then their keys, first, last and power
   const void *key = nullptr, *first = nullptr, *last = nullptr, *power = nullptr;
+  bool has_lead = false;  // B2S_FLAG_SUBFRAME_OVERLAP: whether the next push's frame 0 has a lead-in, and its N / 2 samples
+  const void* lead = nullptr;
 };
 
 template <class IO>
@@ -319,6 +322,13 @@ void band_sections(IO& io, BandImage& s, std::vector<b2s_transmission>& mailbox,
   list<uint64_t>(
       io, rows, "the spectrogram row section is malformed", [&](auto& io, auto& r) { io(r.time), io(r.center), io.bytes(r.row, M); }, M > 0 ? UINT64_MAX : 0);
   io.close("the spectrogram row section has the wrong length");
+
+  // only a band with overlapping sub-frames has this section; a load has checked that the snapshot's overlap bit is the band's
+  if (own.flags & B2S_FLAG_SUBFRAME_OVERLAP) {
+    io.open("LEAD", "the lead-in section is missing or truncated");
+    io.flag(s.has_lead), io.array(s.lead, static_cast<size_t>(n / 2) * (own.iq_format == B2S_IQ_CS8 ? 2 : 8));
+    io.close("the lead-in section has the wrong length");
+  }
 }
 
 // ---- recorder bank: CONF RAWC, then one CHAN per channel ----

@@ -180,18 +180,32 @@ struct SpectralArgs {
   const float2* split_ws;       // [S]         W_S^j
   unsigned long long* peak_packed;  // [n_frames], zeroed before the launch: max over the S classes of (ordered(value) << 32 | ~index)
   // ---- sub-frames (the SUB instantiations only, B2S_FLAG_SUBFRAME_*) ----
-  int sub_r;                    // sub-frames per frame, r >= 2: sub-frame j starts at iq + k * frame_stride_bytes + j * N samples
-  int sub_max;                  // reduction over the sub-frames' |X|^2/fs: 0 = mean (sum in order, then / r), 1 = maximum
+  int sub_r;                    // sub-frames per frame, >= 2: sub-frame j of frame k starts at
+                                //   iq + k * frame_stride_bytes + sub_off_bytes + j * sub_step_bytes
+  int sub_max;                  // reduction over the sub-frames' |X|^2/fs: 0 = mean (sum in order, then / count), 1 = maximum
+  long long sub_step_bytes;     // N samples back to back; N / 2 samples with B2S_FLAG_SUBFRAME_OVERLAP
+  long long sub_off_bytes;      // 0; -N / 2 samples with the overlap (sub-frame 0 straddles the previous frame's end)
+  // overlap: frame 0's sub-frame 0 is read from sub_lead (N contiguous samples: the lead-in, then the launch's first N / 2),
+  // never from before iq; sub_first = 1 drops it (no lead-in) and frame 0 folds sub-frames 1 ... sub_r - 1
+  const void* sub_lead;
+  int sub_first;
 };
 
+// The first sub-frame a frame folds: 0, or a.sub_first for frame 0
+__device__ __forceinline__ int sub_begin(const SpectralArgs& a, long long frame) { return frame == 0 ? a.sub_first : 0; }
+// First sample of sub-frame `sub` of `frame`
+__device__ __forceinline__ const char* sub_src(const SpectralArgs& a, const char* base, long long frame, int sub) {
+  if (frame == 0 && sub == 0 && a.sub_lead) return static_cast<const char*>(a.sub_lead);
+  return base + frame * a.frame_stride_bytes + a.sub_off_bytes + static_cast<long long>(sub) * a.sub_step_bytes;
+}
 // One sub-frame's |X|^2/fs folded into the frame's partial: MEAN adds in sub-frame order, MAX keeps the larger. On the last
-// sub-frame the caller divides the mean by r.
-__device__ __forceinline__ float sub_fold(float part, float pw, int sub, int sub_max) {
-  if (sub == 0) return pw;
+// sub-frame the caller divides the mean by the number of sub-frames folded.
+__device__ __forceinline__ float sub_fold(float part, float pw, bool first, int sub_max) {
+  if (first) return pw;
   return sub_max ? fmaxf(part, pw) : __fadd_rn(part, pw);
 }
-__device__ __forceinline__ float sub_finish(float acc, const SpectralArgs& a) {
-  return a.sub_max ? acc : __fdiv_rn(acc, static_cast<float>(a.sub_r));
+__device__ __forceinline__ float sub_finish(float acc, const SpectralArgs& a, int count) {
+  return a.sub_max ? acc : __fdiv_rn(acc, static_cast<float>(count));
 }
 
 // tw points at this pass's [m-1][k] table (shared or global)
@@ -256,6 +270,7 @@ __device__ __forceinline__ float fast_log2(float x) {
 // SUB (B2S_FLAG_SUBFRAME_*): a frame is a_.sub_r sub-frames of N samples, transformed one after the other by the CTA that takes
 // the frame; the TMA buffer is filled with the next sub-frame (or the next frame's first) behind each pass 0. The thread that owns
 // bin b in the epilogue folds every sub-frame's |X|^2/fs into acc[] (registers) and the last sub-frame converts the reduced row.
+// Where the sub-frames lie (back to back, or overlapping by half with frame 0's first one from a.sub_lead) is sub_src's.
 template <int N, int MODE, bool DEBUG_LIN, bool SUB>
 __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralArgs a) {
   using PL = FftPlanT<N>;
@@ -280,9 +295,8 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
   const char* base = static_cast<const char*>(a.iq);
   // first sample of sub-frame `sub` of `frame` (sub = 0 without SUB)
   auto src = [&](long long frame, int sub) {
-    const char* p = base + frame * a.frame_stride_bytes;
-    if (SUB) p += static_cast<long long>(sub) * N * (MODE == kModeCf32 ? 8 : 2);
-    return p;
+    if (SUB) return sub_src(a, base, frame, sub);
+    return base + frame * a.frame_stride_bytes;
   };
 
   if (MODE == kModeCs8Tma) {
@@ -308,7 +322,7 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
   if (MODE == kModeCs8Tma) {
     if (tid == 0 && static_cast<int>(blockIdx.x) < a.n_frames) {
       mbar_arrive_expect_tx(&full_bar, 2 * N);
-      bulk_g2s(raw, src(blockIdx.x, 0), 2 * N, &full_bar);
+      bulk_g2s(raw, src(blockIdx.x, SUB ? sub_begin(a, blockIdx.x) : 0), 2 * N, &full_bar);
     }
   }
 
@@ -316,7 +330,9 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
   for (int frame = blockIdx.x; frame < a.n_frames; frame += gridDim.x) {
     float2 v[E];
     float acc[SUB ? E : 1];  // SUB: the frame's partial reduction of the bins this thread owns in the epilogue
-    for (int sub = 0; sub < (SUB ? a.sub_r : 1); ++sub) {
+    const int sub0 = SUB ? sub_begin(a, frame) : 0;
+    for (int sub = sub0; sub < (SUB ? a.sub_r : 1); ++sub) {
+    const char* sub_p = SUB ? src(frame, sub) : nullptr;  // SUB: the sub-frame's first sample, once per sub-frame
     // ---------------- pass 0: unpack + window, radix R0, no twiddles (P = 1) ----------------
     {
       constexpr int NB = N / R0, BPT = E / R0;
@@ -333,10 +349,10 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
             const char2 s = reinterpret_cast<const char2*>(raw)[n];
             v[u * R0 + m] = make_float2(static_cast<float>(s.x) * w, static_cast<float>(s.y) * w);
           } else if (MODE == kModeCs8Direct) {
-            const signed char* fp = reinterpret_cast<const signed char*>(src(frame, sub));
+            const signed char* fp = reinterpret_cast<const signed char*>(SUB ? sub_p : src(frame, sub));
             v[u * R0 + m] = make_float2(static_cast<float>(fp[2 * n]) * w, static_cast<float>(fp[2 * n + 1]) * w);
           } else {
-            const float* fp = reinterpret_cast<const float*>(src(frame, sub));
+            const float* fp = reinterpret_cast<const float*>(SUB ? sub_p : src(frame, sub));
             v[u * R0 + m] = make_float2(fp[2 * n] * w, fp[2 * n + 1] * w);
           }
         }
@@ -351,7 +367,7 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
         mbar_arrive_expect_tx(&full_bar, 2 * N);
         bulk_g2s(raw, src(frame, sub + 1), 2 * N, &full_bar);
       } else {
-        const int next = frame + gridDim.x;
+        const int next = frame + gridDim.x;  // > 0: starts at its sub-frame 0
         if (next < a.n_frames) {
           mbar_arrive_expect_tx(&full_bar, 2 * N);
           bulk_g2s(raw, src(next, 0), 2 * N, &full_bar);
@@ -379,7 +395,7 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
     pass_twiddle_butterfly<N, RL, PL_, E, T>(v, NP == 4 ? tw3 : (NP == 3 ? tw2 : tw1), tid);
     if (SUB) {
 #pragma unroll
-      for (int i = 0; i < E; ++i) acc[i] = sub_fold(acc[i], fmaf(v[i].x, v[i].x, v[i].y * v[i].y) * a.inv_fs, sub, a.sub_max);
+      for (int i = 0; i < E; ++i) acc[i] = sub_fold(acc[i], fmaf(v[i].x, v[i].x, v[i].y * v[i].y) * a.inv_fs, sub == sub0, a.sub_max);
       if (sub + 1 < a.sub_r) __syncthreads();  // every thread has read X before the next sub-frame's pass 0 overwrites it
     }
     }
@@ -397,7 +413,7 @@ __global__ void __launch_bounds__(N / FftPlanT<N>::E) k_spectrum(const SpectralA
         for (int m = 0; m < RL; ++m) {
           const float2 z = v[u * RL + m];
           const int j = (b + m * NB + N / 2) & (N - 1);
-          const float pw = SUB ? sub_finish(acc[u * RL + m], a) : fmaf(z.x, z.x, z.y * z.y) * a.inv_fs;
+          const float pw = SUB ? sub_finish(acc[u * RL + m], a, a.sub_r - sub0) : fmaf(z.x, z.x, z.y * z.y) * a.inv_fs;
           const float db = kDbPerLog2 * fast_log2(pw);
           row[j] = db;
           if (DEBUG_LIN) a.power_lin[static_cast<size_t>(frame) * N + j] = pw;

@@ -128,7 +128,8 @@ constexpr int kSplitStageBytes = 32768; // one staging buffer: S row segments of
 // mode, is staged while j is transformed). The thread that owns a bin after pass C folds each sub-frame's |X|^2/fs into the
 // partial it keeps at that bin's place in the item's own psd_db row: the same thread writes and rereads the same addresses, so
 // no barrier or atomic is needed, and the row stays in L2. The last sub-frame reads the partial, finishes the reduction, and runs
-// the dB conversion, the stores and the first-maximum search of a frame without sub-frames on the reduced row.
+// the dB conversion, the stores and the first-maximum search of a frame without sub-frames on the reduced row. Where the
+// sub-frames lie is sub_src's; the items of frame 0 start at sub_begin (1 when an overlapping frame 0 has no lead-in).
 template <int RA, int MODE, bool DEBUG_LIN, int SPLIT_S, bool SUB>
 __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
   constexpr bool SPLIT = SPLIT_S > 1;
@@ -167,10 +168,11 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
 
   // first sample of sub-frame `sub` of `frame` (sub = 0 without SUB)
   auto frame_src = [&](int frame, int sub) {
-    const char* p = base + static_cast<long long>(frame) * a.frame_stride_bytes;
-    if (SUB) p += static_cast<long long>(sub) * N * (MODE == kModeCf32 ? 8 : 2);
-    return p;
+    if (SUB) return sub_src(a, base, frame, sub);
+    return base + static_cast<long long>(frame) * a.frame_stride_bytes;
   };
+  // the sub-frame an item starts at: 0, or a.sub_first for frame 0's items
+  auto sub_begin_of = [&](int it_) { return SUB ? sub_begin(a, SPLIT ? it_ / S : it_) : 0; };
   // stage `q`-th chunk of sub-frame `sub` of `it_`: S segments [s][pc samples] of the frame (split) / the whole frame (non-split)
   auto issue = [&](int it_, int sub, int q, int stage) {
     if (SPLIT) {
@@ -184,8 +186,8 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
     }
   };
   if (MODE == kModeCs8Tma && tid == 0 && item < n_items) {
-    issue(item, 0, 0, 0);
-    if (SPLIT) issue(item, 0, 1, 1);
+    issue(item, sub_begin_of(item), 0, 0);
+    if (SPLIT) issue(item, sub_begin_of(item), 1, 1);
   }
 
   constexpr bool kDefer = !SPLIT;
@@ -195,11 +197,13 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
   uint32_t parity = 0;   // non-split: phase of full_bar[0]
   uint32_t chunk_no = 0; // split: chunks consumed so far by this CTA (stage = chunk_no & 1, phase = (chunk_no >> 1) & 1)
   int round = 0;
-  int sub = 0;           // SUB: the sub-frame of `item` in hand
+  int sub = sub_begin_of(item);  // SUB: the sub-frame of `item` in hand
   while (item < n_items) {
     const int frame = SPLIT ? item / S : item;
     const int c = SPLIT ? item - frame * S : 0;
-    const bool first_sub = !SUB || sub == 0;
+    const int sub0 = sub_begin_of(item);
+    const bool first_sub = !SUB || sub == sub0;
+    const char* sub_p = SUB ? frame_src(frame, sub) : nullptr;  // SUB: the sub-frame's first sample, once per sub-frame
     if (tid == 0 && first_sub) s_item[(round + 1) & 1] = atomicAdd(a.work_counter, 1);  // the item after this one (read after the next barrier)
     if (tid == 32 && c == 0 && first_sub) {  // K2's per-frame counters (SpectralArgs::zero_per_frame)
       if (a.zero_per_frame[0]) a.zero_per_frame[0][frame] = 0;
@@ -222,10 +226,10 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
             const char2 smp = reinterpret_cast<const char2*>(st + s * pc * 2)[i];
             return cscale(cmake(C{}, static_cast<float>(smp.x), static_cast<float>(smp.y)), w);
           } else if (MODE == kModeCs8Direct) {
-            const signed char* fp = reinterpret_cast<const signed char*>(frame_src(frame, sub));
+            const signed char* fp = reinterpret_cast<const signed char*>(SUB ? sub_p : frame_src(frame, sub));
             return cscale(cmake(C{}, static_cast<float>(fp[2 * n]), static_cast<float>(fp[2 * n + 1])), w);
           } else {
-            const float* fp = reinterpret_cast<const float*>(frame_src(frame, sub));
+            const float* fp = reinterpret_cast<const float*>(SUB ? sub_p : frame_src(frame, sub));
             return cscale(cmake(C{}, fp[2 * n], fp[2 * n + 1]), w);
           }
         };
@@ -269,7 +273,7 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
           const int next = s_item[(round + 1) & 1];
           if (q + 2 < S) issue(item, sub, q + 2, chunk_no & 1u);
           else if (SUB && sub + 1 < a.sub_r) issue(item, sub + 1, q + 2 - S, chunk_no & 1u);
-          else if (next < n_items) issue(next, 0, q + 2 - S, chunk_no & 1u);
+          else if (next < n_items) issue(next, sub_begin_of(next), q + 2 - S, chunk_no & 1u);
         }
         ++chunk_no;
       }
@@ -297,11 +301,11 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
             v0[m] = cscale(cmake(C{}, static_cast<float>(s.x), static_cast<float>(s.y)), w.x);
             v1[m] = cscale(cmake(C{}, static_cast<float>(s.z), static_cast<float>(s.w)), w.y);
           } else if (MODE == kModeCs8Direct) {
-            const signed char* fp = reinterpret_cast<const signed char*>(frame_src(frame, sub)) + 2 * n;
+            const signed char* fp = reinterpret_cast<const signed char*>(SUB ? sub_p : frame_src(frame, sub)) + 2 * n;
             v0[m] = cscale(cmake(C{}, static_cast<float>(fp[0]), static_cast<float>(fp[1])), w.x);
             v1[m] = cscale(cmake(C{}, static_cast<float>(fp[2]), static_cast<float>(fp[3])), w.y);
           } else {
-            const float2* fp = reinterpret_cast<const float2*>(frame_src(frame, sub)) + n;
+            const float2* fp = reinterpret_cast<const float2*>(SUB ? sub_p : frame_src(frame, sub)) + n;
             const float2 x0 = fp[0], x1 = fp[1];
             v0[m] = cscale(cmake(C{}, x0.x, x0.y), w.x);
             v1[m] = cscale(cmake(C{}, x1.x, x1.y), w.y);
@@ -334,10 +338,10 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
             const char2 s = reinterpret_cast<const char2*>(raw)[n];
             v[m] = cscale(cmake(C{}, static_cast<float>(s.x), static_cast<float>(s.y)), w);
           } else if (MODE == kModeCs8Direct) {
-            const signed char* fp = reinterpret_cast<const signed char*>(frame_src(frame, sub));
+            const signed char* fp = reinterpret_cast<const signed char*>(SUB ? sub_p : frame_src(frame, sub));
             v[m] = cscale(cmake(C{}, static_cast<float>(fp[2 * n]), static_cast<float>(fp[2 * n + 1])), w);
           } else {
-            const float* fp = reinterpret_cast<const float*>(frame_src(frame, sub));
+            const float* fp = reinterpret_cast<const float*>(SUB ? sub_p : frame_src(frame, sub));
             v[m] = cscale(cmake(C{}, fp[2 * n], fp[2 * n + 1]), w);
           }
         }
@@ -356,7 +360,7 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
     const int next_item = s_item[(round + 1) & 1];
     if (!SPLIT && MODE == kModeCs8Tma && tid == 0) {  // staging buffer consumed: fetch the next (sub-)frame behind the remaining passes
       if (SUB && sub + 1 < a.sub_r) issue(item, sub + 1, 0, 0);
-      else if (next_item < n_items) issue(next_item, 0, 0, 0);
+      else if (next_item < n_items) issue(next_item, sub_begin_of(next_item), 0, 0);
     }
     // ---------------- passes B and C: warp `warp` owns block k0 = warp ----------------
     C v[32];
@@ -391,7 +395,7 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
       for (int k2 = 0; k2 < 32; ++k2) {
         const float re = cre(v[k2]), im = cim(v[k2]);
         float& p = part_at(k2);
-        p = sub_fold(p, fmaf(re, re, im * im) * a.inv_fs, sub, a.sub_max);
+        p = sub_fold(p, fmaf(re, re, im * im) * a.inv_fs, first_sub, a.sub_max);
       }
       __syncthreads();  // every warp has read its block before the next sub-frame's pass A overwrites the exchange buffer
       ++sub;
@@ -405,7 +409,7 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
     for (int k2 = 0; k2 < 32; ++k2) {
       const float re = cre(v[k2]), im = cim(v[k2]);
       float pw = fmaf(re, re, im * im) * a.inv_fs;
-      if (SUB) pw = sub_finish(sub_fold(part_at(k2), pw, sub, a.sub_max), a);
+      if (SUB) pw = sub_finish(sub_fold(part_at(k2), pw, first_sub, a.sub_max), a, a.sub_r - sub0);
       const float db = kDbPerLog2 * fast_log2(pw);
       res[k2 * 32 + lane] = DEBUG_LIN ? pw : db;
       best_v = fmaxf(best_v, db);
@@ -502,7 +506,7 @@ __global__ void __launch_bounds__(RA * 32) k_spectrum3(const SpectralArgs a) {
     }
     item = next_item;
     ++round;
-    sub = 0;
+    sub = sub_begin_of(item);
   }
   if (kDefer) {
     __syncthreads();
